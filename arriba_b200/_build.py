@@ -1,6 +1,6 @@
 """Build logic for arriba-b200 (used by __graft_entry__.build(), the tests and bench.py).
 
-product : nvcc -gencode arch=compute_100a,code=sm_100a  -> arriba_b200/libarriba_b200.so   (CUDA, the only library the package loads)
+product : nvcc -gencode arch=compute_90a,code=sm_90a  -> arriba_b200/libarriba_b200.so   (CUDA, the only library the package loads)
 hostsim : g++ -DARB_HOSTSIM over the same sources       -> tests/hostsim/libarriba_b200_hostsim.so (CPU test-suite only)
 oracle  : oracle/Makefile (unmodified reference + shim) -> oracle/_ref/arriba               (only when /root/reference exists)
 tools   : tools/synth.cpp                                -> build/synth
@@ -19,7 +19,7 @@ REFERENCE = "/root/reference/source"
 
 CU_SOURCES = ["prims.cu", "engine.cu", "bamscan.cu", "annotate.cu", "fusions.cu", "events.cu", "rows.cu", "consensus.cu", "mismap.cu", "exchange.cu", "capi.cu", "selftest.cu"]
 CPP_SOURCES = ["mismatch_table.cpp", "host/refdata.cpp", "host/ingest.cpp", "host/annotate.cpp", "host/viral.cpp", "host/pipeline.cpp", "host/events.cpp", "host/output.cpp", "host/shard.cpp", "host/host_capi.cpp"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--fmad=false",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--fmad=false",
               "-Xcompiler", "-fPIC,-O2,-Wall,-Wno-unused-function", "-Xptxas", "-v"]
 GXX_FLAGS = ["-O2", "-std=c++17", "-fPIC", "-Wall", "-Wno-unused-function", "-ffp-contract=off"]
 
@@ -55,7 +55,7 @@ def nvcc_path():
 
 
 def build_product(force=False, verbose=False):
-    """Cross-compiles every CUDA source for sm_100a (works without a GPU) and links the C-ABI shared library."""
+    """Cross-compiles every CUDA source for sm_90a (works without a GPU) and links the C-ABI shared library."""
     if not force and not _newer(PRODUCT_LIB, _all_sources()):
         return PRODUCT_LIB
     objdir = os.path.join(ROOT, "build", "product")
@@ -72,7 +72,7 @@ def build_product(force=False, verbose=False):
     with ThreadPoolExecutor(8) as ex:
         list(ex.map(lambda c: _run(c, log), jobs))
     objs = [os.path.join(objdir, s.replace("/", "_") + ".o") for s in CU_SOURCES + CPP_SOURCES]
-    _run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", PRODUCT_LIB] + objs + ["-lcudart", "-lz", "-lpthread"], log)
+    _run([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", PRODUCT_LIB] + objs + ["-lcudart", "-lz", "-lpthread"], log)
     with open(os.path.join(objdir, "build.log"), "w") as f:
         f.write("\n".join(log))
     if verbose:

@@ -35,7 +35,7 @@ extern "C" {
 
 const char* arb_backend(void) {
 #ifdef ARB_DEVICE_BUILD
-	return "cuda-sm_100a";
+	return "cuda-sm_90a";
 #else
 	return "hostsim-TEST-ONLY";
 #endif
@@ -55,7 +55,7 @@ int arb_ctx_create(arb_ctx** out, int device) {
 		ARB_CUDA_CHECK(cudaSetDevice(device));
 		cudaDeviceProp prop;
 		ARB_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-		if (prop.major < 10) throw arb_error(std::string("device '") + prop.name + "' is not sm_100-class; this build targets sm_100a only");
+		if (prop.major != 9 || prop.minor != 0) throw arb_error(std::string("device '") + prop.name + "' is not sm_90 (Hopper); this build targets sm_90a only");
 #else
 		(void) device;
 #endif

@@ -1,7 +1,7 @@
 // hd.h -- host/device portability layer for arriba-b200.
 //
 // Every per-fragment / per-candidate rule of the hot path is written once as an ARB_HD functor.
-// The product compiles them with nvcc for sm_100a and launches them as CUDA kernels (prims.cuh).
+// The product compiles them with nvcc for sm_90a and launches them as CUDA kernels (prims.cuh).
 // The SAME functors can be compiled by g++ with -DARB_HOSTSIM into a separate, test-only library
 // (tests/hostsim) so that rule logic can be checked against the oracle on machines without a GPU;
 // the product library never contains or falls back to that build.

@@ -34,7 +34,7 @@ static const char* FILTERS[] = {"", "duplicates", "inconsistently_clipped", "hom
 	"uninteresting_contigs", "viral_contigs", "top_expressed_viral_contigs", "low_coverage_viral_contigs", "genomic_support", "isoforms", "low_entropy", "homologs"};
 
 static void usage() {
-	std::cout << "arriba-b200: B200-native implementation of Arriba's post-alignment path (reference version 2.5.1 semantics)\n\n"
+	std::cout << "arriba-b200: H100-native implementation of Arriba's post-alignment path (reference version 2.5.1 semantics)\n\n"
 	          << "Usage: arriba -x Aligned.out.bam -g annotation.gtf -a assembly.fa -o fusions.tsv [-O fusions.discarded.tsv] [OPTIONS]\n\n"
 	          << " -x FILE  BAM with main and chimeric alignments (STAR --chimOutType WithinBAM)\n -g FILE  gene annotation (GTF)\n -a FILE  assembly (FastA)\n"
 	          << " -o FILE  output file   -O FILE  discarded candidates\n -f LIST  disable filters (comma/space separated)\n -s MODE  strandedness auto|yes|no|reverse\n"

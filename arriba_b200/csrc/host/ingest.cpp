@@ -199,8 +199,8 @@ struct worker {
 	void park_waiting() { if (waiting_ptr) { pending.emplace(waiting_key, std::vector<u8>(waiting_ptr, waiting_ptr + waiting_size)); waiting_ptr = NULL; } } // before the chunk buffer is recycled
 	std::vector<final_frag> keep; // the fragments that survive slot normalisation, with their name prefixes
 	worker(): cov(NULL), waiting_ptr(NULL), waiting_size(0), last_fragment(0xFFFFFFFFu), mapped_reads(0), malformed(0), missing_hi(0), records(0), no_chimeric(true), key_hash_hint(0) {}
-	// A worker's pools are gigabytes that a sample touches for the first time page by page (a tenth of the ingest's CPU time went into those faults, tools/hostprof
-	// on the GPU box): the workers of a finished sample are kept for the next one -- contents dropped, memory kept (arb_release_host_memory gives it back).
+	// A worker's pools are gigabytes that a sample touches for the first time page by page (the page faults are a visible share of the ingest's CPU time,
+	// tools/hostprof shows them): the workers of a finished sample are kept for the next one -- contents dropped, memory kept (arb_release_host_memory gives it back).
 	void recycle() {
 		names.clear(); cigars.clear(); seqs.clear(); alns.clear(); frags.clear(); norm_alns.clear(); norm_cigars.clear(); keep.clear(); pending.clear(); viral_reads.clear();
 		std::fill(name_slots.begin(), name_slots.end(), 0u);

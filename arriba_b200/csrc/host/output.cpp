@@ -902,8 +902,8 @@ struct writer {
 		const u64 total = at[n_chunks] + blob_bytes;
 		// a regular file is sized once and filled through a shared mapping by all threads (buffered write() calls to ONE file serialise on its inode lock);
 		// anything else (a pipe, /dev/stdout) gets one sequential writer
-		// Measured on the GPU box (profiles/r02p/writebench.txt, overlay file system): one thread calling write() with 8 MiB pieces moves 5.5 GB/s into the page
-		// cache, a shared mapping filled by 16 threads 1.7-3 GB/s (a page fault per 4 KiB of a fresh file). The mapping stays available as ARB_WRITER_MMAP=1.
+		// On an overlay file system one thread calling write() with 8 MiB pieces fills the page cache faster than a shared mapping filled by 16 threads (a page
+		// fault per 4 KiB of a fresh file; tools/writebench.cpp compares the two). The mapping stays available as ARB_WRITER_MMAP=1.
 		void* map = MAP_FAILED;
 		struct stat st;
 		if (getenv("ARB_WRITER_MMAP") && atoi(getenv("ARB_WRITER_MMAP")) != 0 && ::fstat(fd, &st) == 0 && S_ISREG(st.st_mode) && total > 0 && ::ftruncate(fd, (off_t) total) == 0) map = ::mmap(NULL, total, PROT_READ | PROT_WRITE, MAP_SHARED, fd, 0);

@@ -199,7 +199,7 @@ void engine::filter_mismappers_part(i32 max_mate_gap, int part, int parts, void*
 	auto launch = [&](u32 n, const auto& fn) { if (mismap_min_blocks >= 4) for_each_occ<4>(ex, n, fn); else if (mismap_min_blocks == 3) for_each_occ<3>(ex, n, fn); else for_each(ex, n, fn); };
 	if (mismap_group_pass) {
 #ifdef ARB_DEVICE_BUILD
-		if (I) { // lanes per work item (ARB_MISMAP_GROUP_LANES): 16 measured best on the default workload (profiles/r02i: 204 / 189 / 191 ms with 8 / 16 / 32)
+		if (I) { // lanes per work item (ARB_MISMAP_GROUP_LANES, default 16)
 			if (mismap_group_lanes >= 32) launch_mismap_items<32>(ex, items, I, mismap_budget, heavy.ptr(), n_heavy.ptr());
 			else if (mismap_group_lanes >= 16) launch_mismap_items<16>(ex, items, I, mismap_budget, heavy.ptr(), n_heavy.ptr());
 			else launch_mismap_items<8>(ex, items, I, mismap_budget, heavy.ptr(), n_heavy.ptr());

@@ -1,4 +1,4 @@
-// prims.cu -- hand-written sm_100a implementations of the primitives declared in prims.h
+// prims.cu -- hand-written sm_90a implementations of the primitives declared in prims.h
 // (exclusive scan, stable LSD radix sort). HBM-bound integer kernels: coalesced 128-bit loads, shared-memory
 // staging, warp shuffles / match; no tensor-core work and no library calls.
 #include "prims.h"

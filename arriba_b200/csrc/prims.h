@@ -2,7 +2,7 @@
 // stable LSD radix sort of (key,value) pairs, and an exact "group by key, smallest index wins" hash index.
 //
 // Two builds of the SAME interface:
-//   * product (nvcc, sm_100a): hand-written CUDA kernels below (#ifdef ARB_DEVICE_BUILD). No CUB/Thrust.
+//   * product (nvcc, sm_90a): hand-written CUDA kernels below (#ifdef ARB_DEVICE_BUILD). No CUB/Thrust.
 //   * tests/hostsim (g++ -DARB_HOSTSIM): sequential stand-ins, used only by the CPU test-suite to check the
 //     per-element rules against the oracle. The product library is never built this way.
 #pragma once

@@ -59,7 +59,7 @@ def ensure_world(name, sample_breakpoints=None):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region, and the card's name and power limit (part of every number measured on it)."""
     def __init__(self, device):
         super().__init__(daemon=True); self.device = device; self.samples = []; self.stop_flag = False
     def run(self):
@@ -73,23 +73,30 @@ class ClockSampler(threading.Thread):
             except Exception:
                 pass
             time.sleep(0.2)
+    def card(self):
+        try:
+            out = subprocess.run(["nvidia-smi", "-i", str(self.device), "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, timeout=5).stdout
+            name, limit = [x.strip() for x in out.strip().split(",")][:2]
+            return {"gpu": name, "power_limit_w": float(limit)}
+        except Exception:
+            return {"gpu": None, "power_limit_w": None}
     def summary(self):
         if not self.samples:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return dict(self.card(), sm_mhz=None, sm_max_mhz=None, reasons=["nvidia-smi unavailable"])
         sm = sorted(int(s[0]) for s in self.samples if s[0].isdigit())
         reasons = set()
         for s in self.samples:
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), s[2:6]):
                 if v.lower().startswith("active"):
                     reasons.add(name)
-        return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": int(self.samples[0][1]) if self.samples[0][1].isdigit() else None, "reasons": sorted(reasons)}
+        return dict(self.card(), sm_mhz=sm[len(sm) // 2] if sm else None, sm_max_mhz=int(self.samples[0][1]) if self.samples[0][1].isdigit() else None, reasons=sorted(reasons))
 
 
 def measured_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not a measured figure"
 
 
 def md5_of(path):
@@ -98,6 +105,29 @@ def md5_of(path):
         for block in iter(lambda: f.read(1 << 24), b""):
             h.update(block)
     return h.hexdigest()
+
+
+DUMP_CANDIDATE_ROWS = 1 << 18   # at most this many candidate rows (a seeded sample beyond it) and
+DUMP_LABELS = 1 << 20           # fragment labels go to --dump-outputs: 37 MB of .npy files at most
+DUMP_COLUMNS = ["contig1", "breakpoint1", "direction1", "contig2", "breakpoint2", "direction2", "gene1", "gene2", "split_reads1", "split_reads2", "discordant_mates",
+                "anchor_start1", "anchor_start2", "filter", "confidence", "evalue"]
+
+
+def dump_outputs(cands, directory):
+    """Writes what one step computed, as a caller of Pipeline receives it (Pipeline.candidates()): the candidate table behind both TSV files, one
+    <column>.npy per column, rows in a canonical order (sorted by every column; the table's own order may differ between builds), and the final
+    fragment labels. Integers go out as float64 (exact), the e-values as float32. Larger tables are sampled with a fixed seed."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    n, labels = int(cands["n"]), cands["labels"]
+    rows = np.lexsort([cands[c] for c in reversed(DUMP_COLUMNS)])   # np.lexsort: the last key is the primary one
+    if n > DUMP_CANDIDATE_ROWS:
+        rows = rows[np.sort(np.random.default_rng(1).choice(n, DUMP_CANDIDATE_ROWS, replace=False))]
+    for c in DUMP_COLUMNS:
+        np.save(os.path.join(directory, "candidates_%s.npy" % c), cands[c][rows].astype(np.float32 if c == "evalue" else np.float64))
+    picked = np.arange(len(labels)) if len(labels) <= DUMP_LABELS else np.sort(np.random.default_rng(2).choice(len(labels), DUMP_LABELS, replace=False))
+    np.save(os.path.join(directory, "fragment_labels.npy"), labels[picked].astype(np.float32))
+    np.save(os.path.join(directory, "counts.npy"), np.array([n, len(labels)], np.float64))   # candidates and fragments before sampling
 
 
 def reference_run(prefix, threads):
@@ -134,11 +164,11 @@ def reference_run(prefix, threads):
     return n, scope_s, total
 
 
-# full-size run of the unmodified reference on the default workload, measured once on the development container (profiles/cfg2_full_size_parity.txt):
+# full-size runs of the unmodified reference, measured once on one CPU core of the development container (no GPU involved):
 # the sample above flatters the reference (its std::map / unordered_map walks get slower per fragment as the containers grow)
-REFERENCE_FULL_SIZE = {"cfg2_10M_2x101_50k": {"fragments": 11810114, "seconds": 1535.0, "value": 11810114 / 1535.0, "cores": 1, "where": "development container, profiles/cfg2_full_size_parity.txt (25 min 35 s)"},
-                       "cfg5_10M_mismapper": {"fragments": 11732540, "seconds": 968.0, "value": 11732540 / 968.0, "cores": 1, "where": "development container, tests/golden/full_size_md5.json (16 min 8 s)"},
-                       "cfg3_15M_2x151_75k": {"fragments": 17587876, "seconds": None, "value": None, "cores": 1, "where": "development container: stopped after 3 h 1 min of CPU time inside filter_mismappers, not finished (profiles/r02z/full_size_host_parity.txt)"}}
+REFERENCE_FULL_SIZE = {"cfg2_10M_2x101_50k": {"fragments": 11810114, "seconds": 1535.0, "value": 11810114 / 1535.0, "cores": 1, "where": "development container, one CPU core (25 min 35 s)"},
+                       "cfg5_10M_mismapper": {"fragments": 11732540, "seconds": 968.0, "value": 11732540 / 968.0, "cores": 1, "where": "development container, one CPU core (16 min 8 s)"},
+                       "cfg3_15M_2x151_75k": {"fragments": 17587876, "seconds": None, "value": None, "cores": 1, "where": "development container: stopped after 3 h 1 min of CPU time inside filter_mismappers, not finished"}}
 
 
 class QuietStderr:
@@ -174,7 +204,10 @@ def main():
     ap.add_argument("--mode", choices=["samples", "sharded"], default="sharded",
                     help="N>1: 'sharded' = ONE sample divided over the ranks (strong scaling, NCCL exchanges); 'samples' = one independent sample per GPU (weak scaling, no collective)")
     ap.add_argument("--no-parity", action="store_true", help="skip the md5 comparison of the output files with the reference's")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write the candidate table and fragment labels of the last step to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
 
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1")); local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     cores = os.cpu_count() or 1
@@ -185,7 +218,7 @@ def main():
             usable = min(cores, max(1.0, float(quota) / float(period)))
     except Exception:
         pass
-    threads_all = args.threads or max(2, min(64, int(round(2 * usable))))                 # 2 threads per usable CPU measured best (profiles/r01i)
+    threads_all = args.threads or max(2, min(64, int(round(2 * usable))))                 # 2 threads per usable CPU
     threads = args.threads or max(2, min(64, int(round(2 * usable / max(1, world)))))   # one sample per rank: the ranks share the host
     wl = WORKLOADS[args.workload]
     sample_bp = args.sample_breakpoints or max(50, int(wl["breakpoints"] * 400000 / wl["fragments"]))  # ~400 k fragments: 10-30 s of reference CPU time
@@ -193,7 +226,7 @@ def main():
     config = {"workload": "synthetic %s: %d fragments 2x%d bp, %d breakpoints, genome %.0f%% of hg38 size (synthetic), %d genes" %
               (args.workload, wl["fragments"], wl["read_length"], wl["breakpoints"], wl["scale"] * 100, wl["genes"]),
               "scope": SCOPE, "value_is": "end to end: BAM on disk -> both TSV files on disk through the public Pipeline API, host<->device copies inside the timed region",
-              "l2": "inputs (>2 GB of SoA columns per step) exceed the 126 MB L2", "host_threads_per_rank": threads, "host_threads_rank0_sharded": threads_all, "host_cpus_usable": usable}
+              "l2": "inputs (>2 GB of SoA columns per step) exceed the 50 MB L2 of an H100", "host_threads_per_rank": threads, "host_threads_rank0_sharded": threads_all, "host_cpus_usable": usable}
 
     if args.impl == "reference":
         if rank != 0:
@@ -234,8 +267,8 @@ def main():
     quiet = QuietStderr(os.path.join(outdir, "library_stderr.log")); quiet.__enter__()
     say = (lambda s: quiet.say(s)) if rank == 0 else (lambda s: None)
 
-    def one_step(sharded):
-        """ingest .. fusions.tsv through the public Pipeline API; returns a dict of what the step measured"""
+    def one_step(sharded, keep_outputs=False):
+        """ingest .. fusions.tsv through the public Pipeline API; returns a dict of what the step measured (and, with keep_outputs, what it computed)"""
         # one sample divided over the ranks: rank 0 does the host work with all host threads, the others only hold a device context
         p = L.Pipeline(prefix + ".bam", prefix + ".gtf", prefix + ".fa", threads=(threads_all if rank == 0 else 2) if sharded else threads, device=local_rank, output=out_tsv, discarded=out_disc)
         if not sharded or rank == 0:
@@ -278,17 +311,18 @@ def main():
         ev = {n: round(st.event_seconds[i], 2) for i, n in enumerate(L.EV_NAMES) if st.event_seconds[i] >= 0.2}
         say("[bench] step: e2e %.2f s, device %.1f ms, ingest %.2f, annotate %.2f, upload %.2f, output %.2f, events >= 0.2 s: %s" %
             (e2e_s, dev_ms, st.seconds[L.STEP_INGEST], st.seconds[L.STEP_ANNOTATE], st.seconds[L.STEP_UPLOAD], st.output_seconds, ev))
+        outputs = p.candidates() if keep_outputs and (rank == 0 or not sharded) else None   # after the clock: rank 0 holds the result of a sharded run
         p.close()
-        return {"n": int(st.n_fragments), "e2e_s": e2e_s, "dev_ms": dev_ms, "st": st, "tm": tm, "d2h": d2h, "n_cand": n_cand, "d2h_parts": d2h_parts, "h2d_parts": h2d_parts}
+        return {"outputs": outputs, "n": int(st.n_fragments), "e2e_s": e2e_s, "dev_ms": dev_ms, "st": st, "tm": tm, "d2h": d2h, "n_cand": n_cand, "d2h_parts": d2h_parts, "h2d_parts": h2d_parts}
 
-    def timed(sharded, warmup, steps):
+    def timed(sharded, warmup, steps, keep_outputs=False):
         for _ in range(warmup):
             one_step(sharded)
         if dist:
             dist.barrier()
         torch.cuda.synchronize()
         t_begin = time.perf_counter()
-        results = [one_step(sharded) for _ in range(steps)]
+        results = [one_step(sharded, keep_outputs and k == steps - 1) for k in range(steps)]
         torch.cuda.synchronize()
         if dist:
             dist.barrier()
@@ -311,7 +345,7 @@ def main():
         for _ in range(args.warmup):
             one_step(sharded)
         launches1 = lib.arb_kernel_launches()
-        results, e2e_s, dev_ms, wall = timed(sharded, 0, args.steps)
+        results, e2e_s, dev_ms, wall = timed(sharded, 0, args.steps, keep_outputs=bool(args.dump_outputs))
     except BaseException:
         import traceback
         quiet.say("bench.py (rank %d): a step failed\n%s" % (rank, traceback.format_exc()))   # on the real stderr, not in the library's log
@@ -341,6 +375,9 @@ def main():
         secondary = {"mode": "sharded" if other else "samples", "scaling": "strong" if other else "weak", "value": r2[0]["n"] * jobs2 / e2, "unit": UNIT, "seconds_per_step": e2, "steps": 2, "warmup": 1,
                      "note": "ONE sample divided over all ranks" if other else "one independent sample per GPU, no collective on the data path"}
     quiet.__exit__()
+    if args.dump_outputs and results[-1]["outputs"] is not None:
+        dump_outputs(results[-1]["outputs"], args.dump_outputs)
+        results[-1]["outputs"] = None
     if rank != 0:
         if dist:
             dist.destroy_process_group()
@@ -350,34 +387,19 @@ def main():
     peak, peak_src = measured_peak()
     jobs = 1 if (sharded or world == 1) else world
 
-    def kernel_entry(name, ms, alg_bytes, unit_note, traffic_key, l2_key=None):
-        traffic = None; t = {}
-        try:
-            t = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-            traffic = t.get(args.workload, {}).get(traffic_key)
-        except Exception:
-            pass
+    def kernel_entry(name, ms, alg_bytes, unit_note):
         ach = alg_bytes / (ms * 1e-3) / 1e9 if ms > 0 else 0.0
-        entry = {"bound": "hbm", "kernel": name, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": traffic, "peak_source": peak_src,
-                 "algorithmic_bytes_per_launch": int(alg_bytes), "kernel_ms": ms, "algorithmic_bytes_are": unit_note}
-        if l2_key:   # explanation for a gather-bound kernel: bytes its loads request from L1/L2 per launch (32-byte sectors, from the same ncu capture) over the live kernel time
-            try:
-                l2 = t.get(args.workload, {}).get(l2_key)
-                if l2 and ms > 0:
-                    entry["l1_l2_request_gbs"] = l2 / (ms * 1e-3) / 1e9
-                    entry["bound_note"] = "gather bound: dependent 4-byte lookups, each a 32-byte sector; DRAM traffic ~ algorithmic bytes, the limiter is the sector rate through L1/L2"
-            except Exception:
-                pass
-        return entry
+        return {"bound": "hbm", "kernel": name, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": None, "peak_source": peak_src,   # traffic: DRAM bytes need a hardware profiler, not measured
+                "algorithmic_bytes_per_launch": int(alg_bytes), "kernel_ms": ms, "algorithmic_bytes_are": unit_note}
 
     mean = lambda f: sum(f(r["tm"]) for r in results) / len(results)
     kernels = [
         kernel_entry("cascade_head (all coordinate / CIGAR / gene-set rules, one launch)", mean(lambda t: t.cascade_head_ms), int(tm.cascade_algorithmic_bytes[0]),
-                     "SURVEY 8(d) column budget of the fragments the launch saw", "cascade_head_dram_bytes"),
+                     "SURVEY 8(d) column budget of the fragments the launch saw"),
         kernel_entry("cascade_sequences (mismatches + low entropy, one launch)", mean(lambda t: t.cascade_sequences_ms), int(tm.cascade_algorithmic_bytes[1]),
-                     "SURVEY 8(d): sequences 3 bit/base + gathered reference 2 bit/base + CIGARs + 11 B/alignment of the queued fragments", "cascade_sequences_dram_bytes"),
+                     "SURVEY 8(d): sequences 3 bit/base + gathered reference 2 bit/base + CIGARs + 11 B/alignment of the queued fragments"),
         kernel_entry("mismappers pass 1 (re-alignment, one launch)", mean(lambda t: t.mismappers_pass1_ms), int(getattr(tm, "mismapper_algorithmic_bytes", 0)),
-                     "SURVEY 8(d): per re-aligned sequence 3l/8 + 8(l-8) + 4*hits + l/2", "mismappers_pass1_dram_bytes", "mismappers_pass1_l2_bytes"),
+                     "SURVEY 8(d): per re-aligned sequence 3l/8 + 8(l-8) + 4*hits + l/2"),
     ]
     dominant = max(kernels, key=lambda k: k["kernel_ms"])
     device_ms = {"annotate": tm.annotate_ms, "order": tm.order_ms, "multimappers": tm.multimappers_ms, "in_vitro": tm.in_vitro_ms, "duplicates": tm.duplicates_ms, "classify": tm.classify_ms, "read_filters_total": tm.read_filters_ms, "find_fusions_total": tm.find_fusions_ms, "h2d": tm.h2d_ms,

@@ -1,4 +1,4 @@
-/* arriba_b200.h -- C ABI of the B200-native implementation of Arriba's post-alignment hot path.
+/* arriba_b200.h -- C ABI of the H100-native (sm_90a) implementation of Arriba's post-alignment hot path.
  *
  * The reference (suhrig/arriba v2.5.1) has no FFI: its seam is the set of C++ free functions that
  * `main` (source/arriba.cpp:79) calls on two in-memory containers. Each entry point below names the
@@ -24,7 +24,7 @@ typedef struct arb_ctx arb_ctx;
 int arb_ctx_create(arb_ctx** out, int device);
 void arb_ctx_destroy(arb_ctx* ctx);
 const char* arb_last_error(arb_ctx* ctx);         /* ctx may be NULL: last error of arb_ctx_create */
-const char* arb_backend(void);                    /* "cuda-sm_100a" for the product library */
+const char* arb_backend(void);                    /* "cuda-sm_90a" for the product library */
 uint64_t arb_kernel_launches(void);               /* kernels launched by this library since load */
 /* sizeof() of the public structs, for bindings to verify their layout: arb_contigs, arb_annotation, arb_params, arb_soa_chunk, arb_candidates,
    arb_evalue_inputs, arb_timings, arb_run_options, arb_run_stats */

@@ -20,7 +20,7 @@ def build():
     with ThreadPoolExecutor(8) as ex:
         list(ex.map(B._run, jobs))
     objs = [os.path.join(ROOT, "build", "product", s + ".o") for s in B.CU_SOURCES] + [os.path.join(objdir, s.replace("/", "_") + ".o") for s in B.CPP_SOURCES]
-    B._run([B.nvcc_path(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_G] + objs + ["-lcudart", "-lz", "-lpthread"])
+    B._run([B.nvcc_path(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB_G] + objs + ["-lcudart", "-lz", "-lpthread"])
     B._run(["gcc", "-O2", "-shared", "-fPIC", "-o", os.path.join(ROOT, "build", "libpcsample.so"), os.path.join(ROOT, "tools", "hostprof", "pcsample.c"), "-ldl"])
     print(LIB_G)
 

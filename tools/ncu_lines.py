@@ -4,7 +4,9 @@ table of the same kernel in the cubin (`nvdisasm -g`), and instructions / thread
 
   ncu_lines.py <report.ncu-rep> <kernel name regex> <file.cubin> [top N]
 The cubin must come from the build that was profiled (cuobjdump -xelf all libarriba_b200.so)."""
-import csv, re, subprocess, sys, collections
+import csv, os, re, subprocess, sys, collections
+
+CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "arriba_b200", "csrc")
 
 
 def main():
@@ -50,7 +52,7 @@ def main():
     for (f, ln), a in sorted(agg.items(), key=lambda kv: -kv[1][2])[:top]:
         if f not in srcs:
             try:
-                srcs[f] = open(subprocess.run(["bash", "-c", "ls /root/repo/arriba_b200/csrc/%s /root/repo/arriba_b200/csrc/host/%s 2>/dev/null | head -1" % (f, f)], stdout=subprocess.PIPE, text=True).stdout.strip()).read().splitlines()
+                srcs[f] = open(next(p for p in (os.path.join(CSRC, f), os.path.join(CSRC, "host", f)) if os.path.exists(p))).read().splitlines()
             except Exception:
                 srcs[f] = []
         text = srcs[f][ln - 1].strip()[:110] if 0 < ln <= len(srcs[f]) else ""

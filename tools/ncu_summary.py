@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Turns ncu output into the small text summaries kept under profiles/.
+"""Turns ncu output into small text summaries.
 
   ncu_summary.py launches <launches.csv>            per-kernel launch count, total/mean time and share of the GPU time
   ncu_summary.py report <file.ncu-rep>              key metrics of every kernel in a `--set full` report (needs ncu on PATH)
