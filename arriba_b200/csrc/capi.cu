@@ -152,6 +152,11 @@ int arb_filter_mismappers_part(arb_ctx* ctx, int32_t max_mate_gap, int part, int
 int arb_filter_mismappers_finish(arb_ctx* ctx, uint64_t* n) { ARB_API_BEGIN(ctx) const uint64_t k = ctx->e.filter_mismappers_finish(); if (n) *n = k; ARB_API_END(ctx) }
 int arb_get_timings(arb_ctx* ctx, arb_timings* out) { ARB_API_BEGIN(ctx) *out = ctx->e.timings; ARB_API_END(ctx) }
 int arb_selftest_mismatch_counts(arb_ctx* ctx, uint32_t* out) { ARB_API_BEGIN(ctx) ctx->e.probe_mismatch_counts(out); ARB_API_END(ctx) } // tests only, not declared in the public header
+int arb_set_genomic_breakpoints(arb_ctx* ctx, uint32_t n, const uint16_t* c1, const uint16_t* c2, const uint8_t* d1, const uint8_t* d2, const int32_t* p1, const int32_t* p2) {
+	ARB_API_BEGIN(ctx) ctx->e.set_genomic_breakpoints(n, c1, c2, d1, d2, p1, p2); ARB_API_END(ctx)
+}
+int arb_mark_genomic_support(arb_ctx* ctx, int32_t max_distance, int32_t max_itd_length, uint32_t* marked) { ARB_API_BEGIN(ctx) const uint32_t m = ctx->e.mark_genomic_support(max_distance, max_itd_length); if (marked) *marked = m; ARB_API_END(ctx) }
+int arb_get_genomic_support(arb_ctx* ctx, int32_t* closest1, int32_t* closest2) { ARB_API_BEGIN(ctx) ctx->e.get_genomic_support(closest1, closest2); ARB_API_END(ctx) }
 int arb_get_slot_swaps(arb_ctx* ctx, uint8_t* out) { ARB_API_BEGIN(ctx) ctx->e.get_slot_swaps(out); ARB_API_END(ctx) }
 
 } // extern "C"

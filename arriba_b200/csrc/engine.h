@@ -75,7 +75,8 @@ struct cand_store {
 	dbuf<u32> gene1, gene2, split_reads1, split_reads2, discordant_mates, list1_off, list2_off, listd_off, list1, list2, listd;
 	dbuf<u16> contig1, contig2; dbuf<i32> bp1, bp2, anchor1, anchor2; dbuf<u8> dir1, dir2, filter, bits, bits2; dbuf<float> evalue;
 	dbuf<u32> first_frag; // fragment whose record created the candidate (merge key of the sharded run)
-	cand_store(): n(0), n_list1(0), n_list2(0), n_listd(0) {}
+	dbuf<i32> closest1, closest2; bool genomic_marked; // closest genomic breakpoints (-d), valid once mark_genomic_support has run on this table
+	cand_store(): n(0), n_list1(0), n_list2(0), n_listd(0), genomic_marked(false) {}
 };
 
 struct exchange_buffer { void* p; u64 bytes; };
@@ -164,6 +165,10 @@ public:
 	void homolog_pairs(const u32* ga, const u32* gb, u32 n, u8* out);
 	u64 filter_mismappers(i32 max_mate_gap);
 	void probe_mismatch_counts(u32* out); // test hook (arb_selftest_mismatch_counts)
+	// genomic breakpoints from whole-genome sequencing (genomic.cu): sorted records + key table, the search writes cands.closest1/2
+	void set_genomic_breakpoints(u32 n, const u16* c1, const u16* c2, const u8* d1, const u8* d2, const i32* p1, const i32* p2);
+	u32 mark_genomic_support(i32 max_distance, i32 max_itd_length); void get_genomic_support(i32* closest1, i32* closest2);
+	dbuf<u64> genomic_key_table; dbuf<u32> genomic_key_begin; dbuf<i32> genomic_pos1, genomic_pos2; u32 genomic_n, genomic_keys, genomic_heavy; bool has_genomic_breakpoints;
 private:
 	read_filter_params make_filter_params();
 	unsigned long genome_size() const;

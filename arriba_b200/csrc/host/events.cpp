@@ -133,7 +133,7 @@ void pipeline::fetch_candidates() {
 	e.n = n;
 	e.gene1.resize(n); e.gene2.resize(n); e.contig1.resize(n); e.contig2.resize(n); e.bp1.resize(n); e.bp2.resize(n); e.dir1.resize(n); e.dir2.resize(n);
 	e.split_reads1.resize(n); e.split_reads2.resize(n); e.discordant_mates.resize(n); e.filter.resize(n); e.bits.resize(n); e.bits2.resize(n);
-	e.anchor1.resize(n); e.anchor2.resize(n); e.evalue.resize(n); e.confidence.assign(n, 0);
+	e.anchor1.resize(n); e.anchor2.resize(n); e.evalue.resize(n); e.confidence.assign(n, 0); e.closest1.clear(); e.closest2.clear();
 	e.list1_off.resize((size_t) n + 1); e.list2_off.resize((size_t) n + 1); e.listd_off.resize((size_t) n + 1);
 	e.list1.resize(n1 + 1); e.list2.resize(n2 + 1); e.listd.resize(nd + 1);
 	arb_candidates c;
@@ -735,7 +735,34 @@ void pipeline::filter_mismappers() { // filter_mismappers.cpp:272-359, on the de
 	log_remaining("Re-aligning chimeric reads to filter fusions with >=80% mis-mappers");
 }
 
-void pipeline::assign_confidence() { // filter_genomic_support.cpp:222-402 (no structural-variant input: closest_genomic_breakpoint = -1)
+// ------------------------------------------------------------------------------------------- genomic support (-d)
+void pipeline::mark_genomic_support() { // filter_genomic_support.cpp:80-220: the file is read here, the search runs on the device (csrc/genomic_hd.h)
+	genomic_records g;
+	read_genomic_breakpoints(opt.genomic_breakpoints_file, ref.contig_ids, g);
+	check(ctx, arb_set_genomic_breakpoints(ctx, (uint32_t) g.pos1.size(), g.contig1.data(), g.contig2.data(), g.dir1.data(), g.dir2.data(), g.pos1.data(), g.pos2.data()), "arb_set_genomic_breakpoints");
+	uint32_t marked = 0;
+	check(ctx, arb_mark_genomic_support(ctx, (int32_t) opt.max_genomic_breakpoint_distance, (int32_t) opt.params.max_itd_length, &marked), "arb_mark_genomic_support");
+	ev.closest1.resize(ev.n); ev.closest2.resize(ev.n);
+	check(ctx, arb_get_genomic_support(ctx, ev.closest1.data(), ev.closest2.data()), "arb_get_genomic_support");
+	std::ostringstream s; s << "Marking fusions with support from whole-genome sequencing in '" << opt.genomic_breakpoints_file << "' (marked=" << marked << ")"; say(s.str());
+}
+
+void pipeline::filter_no_genomic_support() { // filter_genomic_support.cpp:404-419; viral = the -v patterns, not the per-sample verdicts
+	for (u32 k = 0; k < ev.n; ++k)
+		if (ev.filter[k] == F_none && !ev.genomic_support(k) && ev.confidence[k] == 0 && !(ref.contig_flags[ev.contig1[k]] & CF_VIRAL) && !(ref.contig_flags[ev.contig2[k]] & CF_VIRAL))
+			ev.filter[k] = F_no_genomic_support;
+	log_remaining("Filtering low-confidence events with no support from WGS");
+}
+
+void pipeline::recover_genomic_support() { // filter_genomic_support.cpp:421-444
+	for (u32 k = 0; k < ev.n; ++k) {
+		const u8 f = ev.filter[k];
+		if (f != F_none && ev.genomic_support(k) && (f == F_end_to_end || f == F_intronic || f == F_mismappers || f == F_no_coverage || f == F_in_vitro || f == F_relative_support)) ev.filter[k] = F_none;
+	}
+	log_remaining("Searching for fusions with support from WGS");
+}
+
+void pipeline::assign_confidence() { // filter_genomic_support.cpp:222-402
 	// the candidates of every gene (only counted below, so their order does not matter): one CSR table instead of a vector per gene
 	struct gene_list { const u32* p; size_t n; size_t size() const { return n; } u32 operator[](size_t x) const { return p[x]; } };
 	std::vector<u32> by_gene_off(ref.genes.size() + 1, 0), by_gene_items(2 * (size_t) ev.n);
@@ -799,6 +826,11 @@ void pipeline::assign_confidence() { // filter_genomic_support.cpp:222-402 (no s
 			if (s1 + s2 == 0 || s1 + d == 0 || s2 + d == 0) --conf;
 			else if ((s1 + s2) * 20 < d) --conf;
 			else if (ev.evalue[k] > 0.2 || coverage_fraction < 0.01) conf = MEDIUM;
+		}
+		if (conf < HIGH && ev.genomic_support(k)) { // a supporting structural variant (-d)
+			const i32 g1 = ev.closest1[k], g2 = ev.closest2[k];
+			if ((ev.evalue[k] < 0.3 && sup >= 2) || (ev.spliced1(k) && ev.spliced2(k) && ev.gene1[k] != ev.gene2[k]) || std::abs(ev.bp1[k] - g1) + std::abs(ev.bp2[k] - g2) < 20000 ||
+			    ev.contig1[k] != ev.contig2[k] || (std::abs(ev.bp2[k] - ev.bp1[k]) > 1000000 && ev.gene1[k] != ev.gene2[k])) ++conf;
 		}
 		ev.confidence[k] = (u8) conf;
 	});

@@ -25,6 +25,7 @@ struct event_table {
 	column<u32> list1_off, list2_off, listd_off, list1, list2, listd; // CSR, fragment indices in name order
 	std::vector<u32> order; // order[k] = candidate visited k-th by the reference's loops
 	std::vector<u32> rank_of; // inverse of `order`
+	std::vector<i32> closest1, closest2; // closest genomic breakpoints (-d), -1 = none; empty without -d
 	event_table(): n(0) {}
 
 	bool exonic1(u32 k) const { return bits[k] & CB_EXONIC1; }
@@ -36,6 +37,12 @@ struct event_table {
 	u32 n_list2(u32 k) const { return list2_off[k + 1] - list2_off[k]; }
 	u32 n_listd(u32 k) const { return listd_off[k + 1] - listd_off[k]; }
 	bool is_read_through(u32 k) const { return contig1[k] == contig2[k] && bp2[k] - bp1[k] < 400000 && dir1[k] == DOWNSTREAM && dir2[k] == UPSTREAM; } // common.hpp:265-269
+	bool genomic_support(u32 k) const { return !closest1.empty() && closest1[k] >= 0; }
 };
+
+// genomic breakpoints of a -d file (genomic_breakpoints.cpp), normalised so that (contig1, pos1) <= (contig2, pos2), in file order; directions 1 = upstream.
+// Lines that are neither format print the reference's WARNING on stderr.
+struct genomic_records { std::vector<u16> contig1, contig2; std::vector<u8> dir1, dir2; std::vector<i32> pos1, pos2; };
+void read_genomic_breakpoints(const std::string& path, const std::map<std::string, u16>& contigs, genomic_records& out);
 
 }} // namespace

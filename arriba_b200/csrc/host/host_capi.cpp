@@ -2,6 +2,7 @@
 #include <malloc.h>
 #include "pipeline.h"
 #include "index_query.h"
+#include <climits>
 #include <cstring>
 #include <stdexcept>
 
@@ -28,6 +29,7 @@ void arb_default_run_options(arb_run_options* o) {
 	o->min_support = 2; o->min_anchor_length = 23; o->min_spliced_events = 4; o->high_expression_quantile = 0.998f; o->exonic_fraction = 0.33f;
 	o->min_itd_allele_fraction = 0.07f; o->min_itd_support = 10; o->print_extra_info_for_discarded_fusions = 0; o->echo_progress = 0;
 	o->top_viral_contigs = 5; o->viral_contig_min_covered_fraction = 0.05f;
+	o->genomic_breakpoints_file = NULL; o->max_genomic_breakpoint_distance = 100000;
 }
 
 // Dozens of host threads allocate and free at the same time (record parsing, annotation, row formatting). glibc gives every thread its own arena, but arenas
@@ -45,6 +47,7 @@ int arb_pipeline_create(arb_pipeline** out, const arb_run_options* o) {
 	*out = NULL;
 	try {
 		if (!o->bam_file || !o->gtf_file || !o->assembly_file) throw std::runtime_error("bam_file, gtf_file and assembly_file are mandatory");
+		if (o->max_genomic_breakpoint_distance > INT_MAX) throw std::runtime_error("max_genomic_breakpoint_distance must not exceed INT_MAX"); // -D takes 0..INT_MAX (options.cpp:401-403)
 		arb_set_host_memory_device(o->device); // the device whose context page-locks the recycled host blocks
 		arb_pipeline* x = new arb_pipeline();
 		run_options& r = x->p.opt;
@@ -57,6 +60,8 @@ int arb_pipeline_create(arb_pipeline** out, const arb_run_options* o) {
 		r.exonic_fraction = o->exonic_fraction; r.min_itd_allele_fraction = o->min_itd_allele_fraction; r.min_itd_support = o->min_itd_support;
 		r.print_extra_info_for_discarded_fusions = o->print_extra_info_for_discarded_fusions != 0; r.echo_progress = o->echo_progress != 0;
 		r.top_viral_contigs = o->top_viral_contigs; r.viral_contig_min_covered_fraction = o->viral_contig_min_covered_fraction;
+		if (o->genomic_breakpoints_file) r.genomic_breakpoints_file = o->genomic_breakpoints_file;
+		r.max_genomic_breakpoint_distance = o->max_genomic_breakpoint_distance;
 		r.params = o->params; r.strandedness = o->strandedness; r.fragment_length = o->fragment_length; r.threads = o->threads; r.device = o->device;
 		*out = x;
 	} catch (const std::exception& e) { g_pipeline_create_error = e.what(); return 1; }
@@ -158,6 +163,13 @@ int arb_pipeline_candidates(arb_pipeline* x, arb_candidates* c, const uint32_t**
 	if (order) *order = e.order.data();
 	if (confidence) *confidence = e.confidence.data();
 	if (labels) *labels = x->p.labels.data();
+	PIPE_END(x)
+}
+
+int arb_pipeline_genomic_support(arb_pipeline* x, const int32_t** closest1, const int32_t** closest2) {
+	PIPE_BEGIN(x)
+	const event_table& e = x->p.ev;
+	*closest1 = e.closest1.empty() ? NULL : e.closest1.data(); *closest2 = e.closest2.empty() ? NULL : e.closest2.data();
 	PIPE_END(x)
 }
 

@@ -681,6 +681,12 @@ struct writer {
 		for (u32 r = e.listd_off[k]; r < e.listd_off[k + 1] && r < e.listd_off[k] + 8; ++r) __builtin_prefetch(&p.labels[e.listd[r]]);
 	}
 
+	// closest_genomic_breakpoint column (output_fusions.cpp:1195-1205)
+	std::string genomic_breakpoint(u32 contig, i32 bp, i32 genomic) const {
+		if (genomic < 0) return ".";
+		return ref.original_names[contig] + ":" + std::to_string((long long) (genomic + 1)) + "(" + std::to_string((long long) std::abs(bp - genomic)) + ")";
+	}
+
 	// a row with the columns of -X (fusion transcript, peptide, reading frame, read names): every row formatted on the host has them (the discarded file
 	// without -X is formatted on the device, format_discarded_rows_on_device)
 	void format_row(row_buffer& out, u32 k, const side_strings* from_device = NULL) const {
@@ -688,8 +694,9 @@ struct writer {
 			std::string site5 = site(e.gene1[k], e.spliced1(k), e.exonic1(k), e.contig1[k], e.bp1[k]), site3 = site(e.gene2[k], e.spliced2(k), e.exonic2(k), e.contig2[k], e.bp2[k]);
 			u32 g5 = e.gene1[k], g3 = e.gene2[k], c5 = e.contig1[k], c3 = e.contig2[k], d5 = e.dir1[k], d3 = e.dir2[k], s5 = e.split_reads1[k], s3 = e.split_reads2[k];
 			i32 b5 = e.bp1[k], b3 = e.bp2[k]; bool st5 = e.bits[k] & CB_PSTRAND1, st3 = e.bits[k] & CB_PSTRAND2;
+			i32 gb5 = e.closest1.empty() ? -1 : e.closest1[k], gb3 = e.closest2.empty() ? -1 : e.closest2[k];
 			const bool ambiguous = e.bits[k] & CB_PSTRANDS_AMBIGUOUS;
-			if (!(e.bits[k] & CB_TSTART_GENE1)) { std::swap(g5, g3); std::swap(c5, c3); std::swap(d5, d3); std::swap(s5, s3); std::swap(b5, b3); std::swap(st5, st3); std::swap(site5, site3); }
+			if (!(e.bits[k] & CB_TSTART_GENE1)) { std::swap(g5, g3); std::swap(c5, c3); std::swap(d5, d3); std::swap(s5, s3); std::swap(b5, b3); std::swap(st5, st3); std::swap(site5, site3); std::swap(gb5, gb3); }
 			const int cov5 = p.coverage.get_coverage(c5, b5, d5 == UPSTREAM ? DOWNSTREAM : UPSTREAM), cov3 = p.coverage.get_coverage(c3, b3, d3 == UPSTREAM ? DOWNSTREAM : UPSTREAM);
 			std::string tseq = ".", pep = ".", frame = "."; i32 tr5 = -1, tr3 = -1;
 			std::vector<i32> positions;
@@ -711,7 +718,7 @@ struct writer {
 			    << ref.original_names[c5] << ":" << (b5 + 1) << "\t" << ref.original_names[c3] << ":" << (b3 + 1) << "\t" << site5 << "\t" << site3 << "\t"
 			    << fusion_type(k) << "\t" << s5 << "\t" << s3 << "\t" << e.discordant_mates[k] << "\t"
 			    << (cov5 >= 0 ? std::to_string((long long) cov5) : ".") << "\t" << (cov3 >= 0 ? std::to_string((long long) cov3) : ".") << "\t" << CONF[e.confidence[k] & 3] << "\t" << frame
-			    << "\t.\t.\t.\t.";
+			    << "\t.\t.\t" << genomic_breakpoint(c5, b5, gb5) << "\t" << genomic_breakpoint(c3, b3, gb3);
 			// filters column: the candidate's own filter and, with counts, the filters of its supporting reads, in alphabetical order (output_fusions.cpp:1187-1213)
 			unsigned int filter_count[38]; bool filter_present[38];
 			for (int f = 0; f < 38; ++f) { filter_count[f] = 0; filter_present[f] = false; }

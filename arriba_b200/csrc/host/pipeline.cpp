@@ -13,7 +13,7 @@ static double now_s() { return std::chrono::duration<double>(std::chrono::steady
 
 run_options::run_options(): interesting_contigs("1 2 3 4 5 6 7 8 9 10 11 12 13 14 15 16 17 18 19 20 21 22 X Y AC_* NC_*"), viral_contigs("AC_* NC_*"),
 	strandedness(3), fragment_length(200), threads(1), device(0), print_extra_info_for_discarded_fusions(false), min_support(2), min_anchor_length(23), min_spliced_events(4), min_itd_support(10),
-	high_expression_quantile(0.998f), exonic_fraction(0.33f), min_itd_allele_fraction(0.07f), echo_progress(false), top_viral_contigs(5), viral_contig_min_covered_fraction(0.05f) { arb_default_params(&params); }
+	high_expression_quantile(0.998f), exonic_fraction(0.33f), min_itd_allele_fraction(0.07f), echo_progress(false), top_viral_contigs(5), viral_contig_min_covered_fraction(0.05f), max_genomic_breakpoint_distance(100000) { arb_default_params(&params); }
 
 void pipeline::say(const std::string& line) {
 	log += line; log += "\n";
@@ -178,10 +178,11 @@ void pipeline::find_fusions() {
 void pipeline::events_until(int last) { // arriba.cpp:420-545, filters enabled by default
 	const u64 m = opt.params.filter_mask;
 	auto on = [&](int f) { return (m >> f) & 1; };
+	const bool genomic = !opt.genomic_breakpoints_file.empty();
 	for (int s = events_done + 1; s <= last && s < EV_COUNT; ++s) {
 		const double t0 = now_s();
 		switch (s) {
-			case EV_FETCH: fetch_candidates(); break;
+			case EV_FETCH: fetch_candidates(); if (genomic) mark_genomic_support(); break; // arriba.cpp:415-418
 			case EV_MERGE_ADJACENT: if (on(F_merge_adjacent)) merge_adjacent(); break;
 			case EV_MULTIMAPPERS: if (on(F_multimappers)) filter_multimappers(); break;
 			case EV_EVALUE: estimate_evalues(); break;
@@ -196,13 +197,19 @@ void pipeline::events_until(int last) { // arriba.cpp:420-545, filters enabled b
 			case EV_SELECT_BEST: if (on(F_select_best)) select_best(); break;
 			case EV_MARGINAL_READ_THROUGH: if (on(F_marginal_read_through)) filter_marginal_read_through(); break;
 			case EV_MANY_SPLICED: if (on(F_many_spliced)) recover_many_spliced(); break;
-			case EV_SHORT_ANCHOR: if (on(F_short_anchor)) filter_short_anchor(); break;
+			case EV_SHORT_ANCHOR: // arriba.cpp:516-523, then the short-anchor filter
+				if (genomic && on(F_no_genomic_support)) { assign_confidence(); filter_no_genomic_support(); }
+				if (on(F_short_anchor)) filter_short_anchor();
+				break;
 			case EV_END_TO_END: if (on(F_end_to_end)) filter_end_to_end(); break;
 			case EV_NO_COVERAGE: if (on(F_no_coverage)) filter_no_coverage(); break;
 			case EV_KMER_INDEX: if (on(F_homologs) || on(F_mismappers)) make_kmer_index(); break;
 			case EV_HOMOLOGS: if (on(F_homologs)) filter_homologs(); break;
 			case EV_MISMAPPERS: if (on(F_mismappers)) filter_mismappers(); break;
-			case EV_SELECT_BEST2: if (on(F_many_spliced) && on(F_select_best)) select_best(); break; // arriba.cpp:573-579
+			case EV_SELECT_BEST2: // arriba.cpp:567-579
+				if (genomic && on(F_genomic_support)) recover_genomic_support();
+				if (((genomic && on(F_genomic_support)) || on(F_many_spliced)) && on(F_select_best)) select_best();
+				break;
 			case EV_ISOFORMS: if (on(F_isoforms)) recover_isoforms(); break;
 			case EV_CONFIDENCE: assign_confidence(); break;
 		}

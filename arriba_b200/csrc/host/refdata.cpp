@@ -66,7 +66,7 @@ u16 refdata::contig_id(const std::string& name) {
 }
 
 // ------------------------------------------------------------------------------------------- file reading
-static void read_whole_file(const std::string& path, std::string& out) {
+void read_whole_file(const std::string& path, std::string& out) { // autodecompress_file_t (read_compressed_file.cpp:10-45): .gz is inflated whole (gzip and BGZF members)
 	const bool gz = path.size() >= 3 && path.compare(path.size() - 3, 3, ".gz") == 0;
 	out.clear();
 	if (gz) {

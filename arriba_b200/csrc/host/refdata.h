@@ -59,5 +59,6 @@ struct refdata {
 };
 
 std::vector<std::string> read_lines_autodecompress(const std::string& path, std::string& storage);
+void read_whole_file(const std::string& path, std::string& out);
 
 }} // namespace

@@ -46,6 +46,7 @@ void engine::format_discarded_rows(const u8* confidence, u64* n_rows, u64* n_byt
 	fm.t.gene_name.chars = row_gene_name.ptr(); fm.t.gene_name.off = row_gene_name_off.ptr(); fm.t.gene_id.chars = row_gene_id.ptr(); fm.t.gene_id.off = row_gene_id_off.ptr();
 	fm.t.contig_name.chars = row_contig_name.ptr(); fm.t.contig_name.off = row_contig_name_off.ptr(); fm.t.filter_name.chars = row_filter_name.ptr(); fm.t.filter_name.off = row_filter_name_off.ptr();
 	fm.t.exon_prev = row_exon_prev.ptr(); fm.t.exon_next = row_exon_next.ptr(); fm.t.confidence = conf.ptr();
+	fm.t.closest1 = cands.genomic_marked ? cands.closest1.ptr() : NULL; fm.t.closest2 = cands.genomic_marked ? cands.closest2.ptr() : NULL;
 	fm.t.cov.windows = coverage_windows.ptr(); fm.t.cov.contig_off = coverage_off.ptr(); fm.t.cov.contig_windows = coverage_n.ptr(); fm.t.cov.n_contigs = coverage_contigs;
 	for (int k = 0; k < ARB_N_FILTERS; ++k) fm.t.filters_by_name[k] = row_filters_by_name[k];
 	fm.t.max_itd_length = row_max_itd_length;

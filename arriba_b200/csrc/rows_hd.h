@@ -19,6 +19,7 @@ struct row_tables { // what the rows need besides the candidate state, the fragm
 	text_pool gene_name, gene_id, contig_name, filter_name;
 	const i32* exon_prev; const i32* exon_next;   // neighbours in the transcript (-1: none)
 	const u8* confidence;                          // per candidate
+	const i32* closest1; const i32* closest2;      // closest genomic breakpoints per candidate (-d), NULL: none marked
 	coverage_view cov;
 	u8 filters_by_name[ARB_N_FILTERS];             // filter ids in alphabetical order of their names
 	u32 max_itd_length;
@@ -93,6 +94,11 @@ struct row_formatter {
 		put_text(w, !f1 ? "duplication/5'-5'" : "duplication/3'-3'");
 	}
 
+	template <class W> ARB_HD void genomic_breakpoint(W& w, u32 contig, i32 bp, i32 genomic) const { // output_fusions.cpp:1195-1205
+		if (genomic < 0) { w.put('.'); return; }
+		put_pool(w, t.contig_name, contig); w.put(':'); put_int(w, (long long) genomic + 1); w.put('(');
+		put_int(w, bp < genomic ? (long long) genomic - bp : (long long) bp - genomic); w.put(')');
+	}
 	template <class W> ARB_HD void strand_column(W& w, bool strand, u32 gene, bool ambiguous) const { w.put(dummy(gene) ? '.' : (forward(gene) ? '+' : '-')); w.put('/'); w.put(ambiguous ? '.' : (strand ? '+' : '-')); }
 
 	// 0 intergenic, 1 intron, 2 3'UTR, 3 5'UTR, 4 exon, 5 UTR, 6 CDS; bit 3: + "/splice-site"   (output_fusions.cpp:635-709)
@@ -143,8 +149,9 @@ struct row_formatter {
 		u32 site5 = site(c.gene1[k], bits & CB_SPLICED1, bits & CB_EXONIC1, c.contig1[k], c.bp1[k]), site3 = site(c.gene2[k], bits & CB_SPLICED2, bits & CB_EXONIC2, c.contig2[k], c.bp2[k]);
 		u32 g5 = c.gene1[k], g3 = c.gene2[k], c5 = c.contig1[k], c3 = c.contig2[k], d5 = c.dir1[k], d3 = c.dir2[k], s5 = c.split_reads1[k], s3 = c.split_reads2[k];
 		i32 b5 = c.bp1[k], b3 = c.bp2[k]; bool st5 = bits & CB_PSTRAND1, st3 = bits & CB_PSTRAND2;
+		i32 gb5 = t.closest1 ? t.closest1[k] : -1, gb3 = t.closest2 ? t.closest2[k] : -1;
 		const bool ambiguous = bits & CB_PSTRANDS_AMBIGUOUS;
-		if (!(bits & CB_TSTART_GENE1)) { u32 x = g5; g5 = g3; g3 = x; x = c5; c5 = c3; c3 = x; x = d5; d5 = d3; d3 = x; x = s5; s5 = s3; s3 = x; const i32 y = b5; b5 = b3; b3 = y; const bool z = st5; st5 = st3; st3 = z; x = site5; site5 = site3; site3 = x; }
+		if (!(bits & CB_TSTART_GENE1)) { u32 x = g5; g5 = g3; g3 = x; x = c5; c5 = c3; c3 = x; x = d5; d5 = d3; d3 = x; x = s5; s5 = s3; s3 = x; i32 y = b5; b5 = b3; b3 = y; const bool z = st5; st5 = st3; st3 = z; x = site5; site5 = site3; site3 = x; y = gb5; gb5 = gb3; gb3 = y; }
 		const int cov5 = t.cov.get(c5, b5, d5 == UPSTREAM ? DOWNSTREAM : UPSTREAM), cov3 = t.cov.get(c3, b3, d3 == UPSTREAM ? DOWNSTREAM : UPSTREAM);
 		gene_name(w, g5, c5, b5); w.put('\t'); gene_name(w, g3, c3, b3); w.put('\t'); strand_column(w, st5, g5, ambiguous); w.put('\t'); strand_column(w, st3, g3, ambiguous); w.put('\t');
 		put_pool(w, t.contig_name, c5); w.put(':'); put_int(w, (long long) b5 + 1); w.put('\t'); put_pool(w, t.contig_name, c3); w.put(':'); put_int(w, (long long) b3 + 1); w.put('\t');
@@ -155,7 +162,8 @@ struct row_formatter {
 		if (cov3 >= 0) put_int(w, cov3); else w.put('.');
 		w.put('\t');
 		switch (t.confidence[k] & 3) { case 0: put_text(w, "low"); break; case 1: put_text(w, "medium"); break; default: put_text(w, "high"); break; }
-		put_text(w, "\t.\t.\t.\t.\t."); // reading frame, tags, retained protein domains, closest genomic breakpoints
+		put_text(w, "\t.\t.\t.\t"); // reading frame, tags, retained protein domains
+		genomic_breakpoint(w, c5, b5, gb5); w.put('\t'); genomic_breakpoint(w, c3, b3, gb3);
 		u32 count[ARB_N_FILTERS]; u64 present = 0;
 		for (u32 x = 0; x < ARB_N_FILTERS; ++x) count[x] = 0;
 		if (c.filter[k] != F_none) present |= (u64) 1 << c.filter[k];

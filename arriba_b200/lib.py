@@ -65,7 +65,8 @@ class Timings(C.Structure):
                 ("merge_adjacent_ms", C.c_float), ("evalue_ms", C.c_float), ("kmer_index_ms", C.c_float), ("homologs_ms", C.c_float), ("mismappers_ms", C.c_float),
                 ("mismapper_items", C.c_uint64), ("kmer_positions", C.c_uint64), ("mismapper_heavy_items", C.c_uint64),
                 ("mismappers_pass1_ms", C.c_float), ("mismappers_pass2_ms", C.c_float), ("mismapper_tasks", C.c_uint64), ("mismapper_rounds", C.c_uint32), ("mismapper_overflow", C.c_uint32), ("mismapper_table_slots", C.c_uint32),
-                ("cascade_head_ms", C.c_float), ("cascade_sequences_ms", C.c_float), ("cascade_queued", C.c_uint64), ("cascade_algorithmic_bytes", C.c_uint64 * 2), ("annotate_ms", C.c_float), ("in_vitro_ms", C.c_float), ("multimappers_ms", C.c_float), ("order_ms", C.c_float), ("partners_ms", C.c_float), ("rows_ms", C.c_float), ("bam_scan_ms", C.c_float), ("consensus_ms", C.c_float), ("mismapper_algorithmic_bytes", C.c_uint64), ("mismapper_sequences", C.c_uint64), ("mismapper_hits", C.c_uint64)]
+                ("cascade_head_ms", C.c_float), ("cascade_sequences_ms", C.c_float), ("cascade_queued", C.c_uint64), ("cascade_algorithmic_bytes", C.c_uint64 * 2), ("annotate_ms", C.c_float), ("in_vitro_ms", C.c_float), ("multimappers_ms", C.c_float), ("order_ms", C.c_float), ("partners_ms", C.c_float), ("rows_ms", C.c_float), ("bam_scan_ms", C.c_float), ("consensus_ms", C.c_float), ("mismapper_algorithmic_bytes", C.c_uint64), ("mismapper_sequences", C.c_uint64), ("mismapper_hits", C.c_uint64),
+                ("genomic_support_ms", C.c_float)]
 
 
 _CTYPE = {np.dtype(np.uint8): C.c_uint8, np.dtype(np.uint16): C.c_uint16, np.dtype(np.uint32): C.c_uint32, np.dtype(np.int32): C.c_int32,
@@ -125,7 +126,9 @@ def load(path=None):
                        ("arb_set_work_partition", [_p(C.c_uint32), _p(C.c_uint8), C.c_uint32, C.c_int, C.c_int]),
                        ("arb_candidates_export", [_p(C.c_void_p), _p(C.c_uint64), _p(C.c_uint64)]), ("arb_candidates_import", [C.c_void_p, C.c_uint64, _p(C.c_uint64), C.c_uint32]),
                        ("arb_swaps_buffer", [_p(C.c_void_p), _p(C.c_uint64)]), ("arb_swaps_apply", []),
-                       ("arb_filter_mismappers_part", [C.c_int32, C.c_int, C.c_int, _p(C.c_void_p), _p(C.c_uint64)]), ("arb_filter_mismappers_finish", [_p(C.c_uint64)])]:
+                       ("arb_filter_mismappers_part", [C.c_int32, C.c_int, C.c_int, _p(C.c_void_p), _p(C.c_uint64)]), ("arb_filter_mismappers_finish", [_p(C.c_uint64)]),
+                       ("arb_set_genomic_breakpoints", [C.c_uint32, _p(C.c_uint16), _p(C.c_uint16), _p(C.c_uint8), _p(C.c_uint8), _p(C.c_int32), _p(C.c_int32)]),
+                       ("arb_mark_genomic_support", [C.c_int32, C.c_int32, _p(C.c_uint32)]), ("arb_get_genomic_support", [_p(C.c_int32), _p(C.c_int32)])]:
         fn = getattr(lib, name)
         fn.argtypes = [C.c_void_p] + args
         fn.restype = C.c_int
@@ -302,6 +305,29 @@ class Context:
         self._check(self.lib.arb_filter_mismappers_finish(self.h, C.byref(n)))
         return int(n.value)
 
+    # ---- genomic breakpoints from whole-genome sequencing (-d)
+    def set_genomic_breakpoints(self, contig1, contig2, direction1, direction2, position1, position2):
+        """Records in file order, each normalised so that (contig1, position1) <= (contig2, position2); directions 1 = upstream."""
+        cols = [np.ascontiguousarray(a, dt) for a, dt in ((contig1, np.uint16), (contig2, np.uint16), (direction1, np.uint8), (direction2, np.uint8), (position1, np.int32), (position2, np.int32))]
+        n = cols[0].size
+        assert all(c.size == n for c in cols), "columns differ in length"
+        cols = [c if c.size else np.zeros(1, c.dtype) for c in cols]
+        self._check(self.lib.arb_set_genomic_breakpoints(self.h, n, *[ptr(c) for c in cols]))
+
+    def mark_genomic_support(self, max_distance=100000, max_itd_length=100):
+        """Closest genomic breakpoints of the resident candidates; returns the number of candidates marked."""
+        m = C.c_uint32()
+        self._check(self.lib.arb_mark_genomic_support(self.h, int(max_distance), int(max_itd_length), C.byref(m)))
+        return int(m.value)
+
+    def genomic_support(self):
+        """(closest_genomic_breakpoint1, closest_genomic_breakpoint2) of every candidate, -1 = none."""
+        n = C.c_uint32()
+        self._check(self.lib.arb_candidates_size(self.h, C.byref(n), None, None, None))
+        a = np.zeros(max(n.value, 1), np.int32); b = np.zeros(max(n.value, 1), np.int32)
+        self._check(self.lib.arb_get_genomic_support(self.h, ptr(a), ptr(b)))
+        return a[:n.value], b[:n.value]
+
     def slot_swaps(self):
         s = np.zeros(self.n_fragments, np.uint8)
         self._check(self.lib.arb_get_slot_swaps(self.h, ptr(s)))
@@ -323,7 +349,8 @@ class RunOptions(C.Structure):
                 ("min_support", C.c_int32), ("min_anchor_length", C.c_uint32), ("min_spliced_events", C.c_uint32), ("high_expression_quantile", C.c_float),
                 ("exonic_fraction", C.c_float), ("min_itd_allele_fraction", C.c_float), ("min_itd_support", C.c_uint32),
                 ("print_extra_info_for_discarded_fusions", C.c_int32), ("echo_progress", C.c_int32),
-                ("top_viral_contigs", C.c_uint32), ("viral_contig_min_covered_fraction", C.c_float)]
+                ("top_viral_contigs", C.c_uint32), ("viral_contig_min_covered_fraction", C.c_float),
+                ("genomic_breakpoints_file", C.c_char_p), ("max_genomic_breakpoint_distance", C.c_uint32)]
 
 
 class RunStats(C.Structure):
@@ -355,6 +382,7 @@ def _load_pipeline_api(lib):
     lib.arb_pipeline_work_partition.argtypes = [C.c_void_p, C.c_int, _p(_p(C.c_uint32)), _p(_p(C.c_uint8)), _p(C.c_uint32)]
     lib.arb_pipeline_mismappers_begin.argtypes = [C.c_void_p, _p(C.c_int)]
     lib.arb_pipeline_mismappers_end.argtypes = [C.c_void_p]
+    lib.arb_pipeline_genomic_support.argtypes = [C.c_void_p, _p(_p(C.c_int32)), _p(_p(C.c_int32))]
     lib._pipeline_ready = True
 
 
@@ -367,7 +395,8 @@ def _np_from(pointer, n, dtype):
 class Pipeline:
     """One run of the hot path on files: the call a user of the library makes (the `arriba` CLI is a thin wrapper over it)."""
 
-    def __init__(self, bam, gtf, fasta, threads=1, device=0, lib_path=None, strandedness=3, params=None, output=None, discarded=None):
+    def __init__(self, bam, gtf, fasta, threads=1, device=0, lib_path=None, strandedness=3, params=None, output=None, discarded=None,
+                 genomic_breakpoints=None, max_genomic_breakpoint_distance=100000):
         self.lib = load(lib_path)
         _load_pipeline_api(self.lib)
         o = RunOptions()
@@ -378,6 +407,9 @@ class Pipeline:
             self._strings.append(output.encode()); o.output_file = self._strings[-1]
         if discarded:
             self._strings.append(discarded.encode()); o.discarded_output_file = self._strings[-1]
+        if genomic_breakpoints:
+            self._strings.append(genomic_breakpoints.encode()); o.genomic_breakpoints_file = self._strings[-1]
+        o.max_genomic_breakpoint_distance = max_genomic_breakpoint_distance
         o.threads = threads; o.device = device; o.strandedness = strandedness
         if params is not None:
             o.params = params
@@ -475,6 +507,10 @@ class Pipeline:
         for k, o in (("list1", "list1_off"), ("list2", "list2_off"), ("listd", "listd_off")):
             out[k] = _np_from(getattr(c, k), int(out[o][-1]) if n else 0, np.uint32)
         out["order"] = _np_from(order, n, np.uint32); out["confidence"] = _np_from(conf, n, np.uint8)
+        g1 = _p(C.c_int32)(); g2 = _p(C.c_int32)()
+        self._check(self.lib.arb_pipeline_genomic_support(self.h, C.byref(g1), C.byref(g2)))
+        out["closest_genomic_breakpoint1"] = _np_from(g1, n, np.int32) if g1 else np.full(n, -1, np.int32)
+        out["closest_genomic_breakpoint2"] = _np_from(g2, n, np.int32) if g2 else np.full(n, -1, np.int32)
         out["labels"] = _np_from(labels, int(self.stats().n_fragments), np.uint8)
         return out
 

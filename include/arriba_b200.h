@@ -297,6 +297,16 @@ int arb_swaps_apply(arb_ctx* ctx);
 int arb_filter_mismappers_part(arb_ctx* ctx, int32_t max_mate_gap, int part, int parts, void** device_verdicts, uint64_t* bytes);
 int arb_filter_mismappers_finish(arb_ctx* ctx, uint64_t* n_realigned);
 
+/* ---- genomic breakpoints from whole-genome sequencing (-d) --------------------------------------------------------------------------------------------------
+ * arb_set_genomic_breakpoints replaces the index that mark_genomic_support (source/filter_genomic_support.cpp:80-167) builds from the file: the parsed records,
+ * each normalised so that (contig1, position1) <= (contig2, position2), in file order (directions 1 = upstream; an INV record of a VCF is two records).
+ * arb_mark_genomic_support replaces its search (:169-219) over the resident candidate table: the closest genomic breakpoint pair of every candidate, -1 = none;
+ * *marked = candidates with closest_genomic_breakpoint1 >= 0. arb_get_genomic_support copies the two columns (n candidates each). */
+int arb_set_genomic_breakpoints(arb_ctx* ctx, uint32_t n, const uint16_t* contig1, const uint16_t* contig2, const uint8_t* direction1, const uint8_t* direction2,
+                                const int32_t* position1, const int32_t* position2);
+int arb_mark_genomic_support(arb_ctx* ctx, int32_t max_distance, int32_t max_itd_length, uint32_t* marked);
+int arb_get_genomic_support(arb_ctx* ctx, int32_t* closest1, int32_t* closest2);
+
 /* ---- device timing (CUDA events recorded on the context's stream around each stage) ---------------------------------- */
 typedef struct arb_timings {
 	float duplicates_ms;        /* duplicate marking (key build + hash group-by + mark) */
@@ -325,6 +335,7 @@ typedef struct arb_timings {
 	float consensus_ms;         /* arb_build_consensus, summed over the batches of the last sample */
 	uint64_t mismapper_algorithmic_bytes; /* SURVEY.md section 8(d) budget of pass 1 of the re-alignment: per searched sequence of length l, 3l/8 + 8(l-8) + 4*hits + l/2 */
 	uint64_t mismapper_sequences, mismapper_hits; /* sequences searched by pass 1 (segment x gene x strand) and k-mer hits they visited */
+	float genomic_support_ms;   /* arb_mark_genomic_support: search of the sorted genomic breakpoints and the copy of the marks */
 } arb_timings;
 int arb_get_timings(arb_ctx* ctx, arb_timings* out);
 /* Device scratch memory is pooled per device and survives arb_ctx_destroy so that the next sample reuses it; this returns it to the driver
@@ -363,6 +374,8 @@ typedef struct arb_run_options {
 	int32_t echo_progress;           /* print the reference's progress lines to stdout while running */
 	uint32_t top_viral_contigs;      /* -T 5 */
 	float viral_contig_min_covered_fraction; /* -C 0.05 */
+	const char* genomic_breakpoints_file;    /* -d: structural variants from whole-genome sequencing (four-column or VCF, optionally .gz), NULL = none */
+	uint32_t max_genomic_breakpoint_distance; /* -D 100000 */
 } arb_run_options;
 void arb_default_run_options(arb_run_options* o);
 
@@ -416,6 +429,8 @@ int arb_pipeline_write_output(arb_pipeline* p);
 /* read-only view of the host candidate table: the arb_candidates pointers alias pipeline memory; `order` = the reference's
    iteration order (candidate ids), `confidence` and the current fragment labels complete the state */
 int arb_pipeline_candidates(arb_pipeline* p, arb_candidates* view, const uint32_t** order, const uint8_t** confidence, const uint8_t** fragment_labels);
+/* closest genomic breakpoints of the candidates (-d; after ARB_EV_FETCH), host columns of n candidates: -1 = none; both NULL when the run has no -d file */
+int arb_pipeline_genomic_support(arb_pipeline* p, const int32_t** closest1, const int32_t** closest2);
 
 #ifdef __cplusplus
 }
