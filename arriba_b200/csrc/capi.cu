@@ -59,10 +59,6 @@ int arb_ctx_create(arb_ctx** out, int device) {
 #else
 		(void) device;
 #endif
-#ifdef ARB_DEVICE_BUILD
-		cudaSetDeviceFlags(cudaDeviceLmemResizeToMax); cudaGetLastError(); // keep the local-memory arena of the recursive re-alignment kernels between launches (best effort)
-		ARB_CUDA_CHECK(cudaDeviceSetLimit(cudaLimitStackSize, 16 * 1024)); // realign() recurses at splice sites and at one deletion (mismap_hd.h)
-#endif
 		*out = new arb_ctx();
 		(*out)->e.device = device;
 	} catch (const std::exception& x) { g_create_error = x.what(); return 1; }

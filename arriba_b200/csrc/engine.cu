@@ -19,12 +19,10 @@ engine::engine(): row_max_itd_length(0), has_row_texts(false), row_text_bytes(0)
 	memset(&timings, 0, sizeof(timings));
 	cons_rows = 0; cons_seq_bytes = cons_pos_count = cons_clip_bytes = 0;
 	// test hooks of the re-alignment passes (mismap_hd.h) that send work through every path: ARB_MISMAP_BUDGET (steps of an item in pass 1 before it goes to
-	// pass 2, 0 = no limit), ARB_MISMAP_LANES (threads per item in pass 2), ARB_MISMAP_SPAWN (steps a continuation may take before it is registered as a task,
-	// 0 = none), ARB_MISMAP_TASK_LANES (threads per task)
-	mismap_budget = 4096; mismap_lanes = 1024; mismap_spawn_budget = 0; mismap_task_lanes = 32;
+	// pass 2, 0 = no limit), ARB_MISMAP_LANES (threads per item in pass 2), ARB_MISMAP_TASK_LANES (threads per task)
+	mismap_budget = 4096; mismap_lanes = 1024; mismap_task_lanes = 32;
 	if (const char* s = getenv("ARB_MISMAP_BUDGET")) mismap_budget = atoi(s);
 	if (const char* s = getenv("ARB_MISMAP_LANES")) mismap_lanes = (u32) std::max(1, atoi(s));
-	if (const char* s = getenv("ARB_MISMAP_SPAWN")) mismap_spawn_budget = atoi(s);
 	homolog_lanes = 32; if (const char* s = getenv("ARB_HOMOLOG_LANES")) homolog_lanes = (u32) std::max(1, atoi(s)); // threads per gene pair in filter_homologs' identity test (1 = one thread per pair)
 	if (const char* s = getenv("ARB_MISMAP_TASK_LANES")) mismap_task_lanes = (u32) std::max(1, atoi(s));
 	ex.scratch = &scratch;
@@ -223,13 +221,6 @@ void engine::finish_push(u64 n_gene_ids) {
 	sequence_bytes = bases * 3 / 8 + bases * 2 / 8 + (push_cigar_ops + n_alignments) * 4 + n_alignments * 11 + (u64) n * 2;
 	timings.classify_algorithmic_bytes = head_bytes + sequence_bytes;
 	push_open = false;
-#ifdef ARB_DEVICE_BUILD
-	{ // realign() (mismap_hd.h) recurses once per continuation, each at least 8 read bases further on, reads of 300 bases and more are not re-aligned: frames of < 512 B
-		const size_t levels = std::min<size_t>(frags.max_seq_len, 300) / 8 + 4, wanted = 1024 + 512 * levels;
-		size_t have = 0;
-		if (cudaDeviceGetLimit(&have, cudaLimitStackSize) == cudaSuccess && have < wanted) ARB_CUDA_CHECK(cudaDeviceSetLimit(cudaLimitStackSize, wanted));
-	}
-#endif
 }
 
 unsigned long engine::genome_size() const { // filter_mismatches.cpp:105-108

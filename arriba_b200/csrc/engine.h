@@ -158,7 +158,7 @@ public:
 	u64 push_alignments, push_bases; u64 head_bytes, sequence_bytes; // column budgets of the two cascade launches for the resident chunk
 	size_t cascade_smem_bytes; u32 cascade_resident_blocks; // launch shape of the sequence kernel on this context's device
 	int device;
-	int mismap_budget, mismap_spawn_budget; u32 mismap_lanes, mismap_task_lanes, homolog_lanes; // work control of the re-alignment passes (mismap_hd.h, realign_ctl)
+	int mismap_budget; u32 mismap_lanes, mismap_task_lanes, homolog_lanes; // work control of the re-alignment passes (mismap_hd.h, realign_ctl)
 	dbuf<u32> splice_off; dbuf<i32> splice_sites; bool has_splice_sites;
 	void set_splice_sites(const u32* off, const i32* sites);
 	u64 build_kmer_index(const u32* contig, const i32* start, const i32* end, u32 n, u32 n_index_contigs);

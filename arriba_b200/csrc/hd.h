@@ -11,11 +11,9 @@
 
 #if defined(__CUDACC__) && !defined(ARB_HOSTSIM)
 #define ARB_HD __host__ __device__ __forceinline__
-#define ARB_HD_RECURSIVE __host__ __device__ inline
 #define ARB_DEVICE_BUILD 1
 #else
 #define ARB_HD inline
-#define ARB_HD_RECURSIVE inline
 #endif
 
 namespace arb {

@@ -197,40 +197,54 @@ void engine::filter_mismappers_part(i32 max_mate_gap, int part, int parts, void*
 	}
 	u32 H = 0; n_heavy.download(ex, &H, 1);
 	stage_timer t2(ex);
-	// pass 2 and the task rounds: continuations are registered per item (mismap_hd.h, realign_ctl::table) and run as tasks, one per distinct continuation
+	// pass 2 and the task rounds: continuations are registered (mismap_hd.h, realign_ctl) and run as tasks, one per distinct continuation
 	// one table for all cooperative items (a read in a long repeat registers thousands of continuations, most reads a handful): 4,096 slots of 16 bytes per
 	// item, at least 2^20 and at most 2^26 slots; the pass 2 kernels keep 4 resident 256-thread blocks per SM (prims.h, for_each_occ)
 	u32 K = 1u << 20; while (K < (1u << 26) && (u64) K < (u64) H * 4096) K <<= 1;
-	if (const char* s = getenv("ARB_MISMAP_TABLE_TOTAL")) { K = 1; while (K < (u32) std::max(1, atoi(s))) K <<= 1; } // test hook: a table that overflows
+	if (const char* s = getenv("ARB_MISMAP_TABLE_TOTAL")) { K = 1; while (K < (u32) std::max(1, atoi(s))) K <<= 1; } // test hook: a first table that overflows
 	if (H >= (1u << 24)) throw arb_error("too many reads need the cooperative re-alignment");
-	dbuf<continuation_slot> tables((size_t) K + 1); dbuf<realign_task> tasks((size_t) K + 1); dbuf<u32> n_tasks(1), overflow(1);
-	overflow.zero(ex, 1);
-	if (H) { continuation_init_fn ci = {tables.ptr()}; for_each(ex, K, ci); }
-	for (u32 done = 0; done < H; ) { // launches of at most 2^31 threads
-		const u32 batch = std::min<u32>(H - done, 0x80000000u / mismap_lanes);
-		mismap_heavy_fn mh = {items, heavy.ptr(), mismap_lanes, mismap_spawn_budget, tables.ptr(), K, done, overflow.ptr()};
-		for_each_occ<4>(ex, batch * mismap_lanes, mh);
-		done += batch;
-	}
-	u64 spawned = 0; u32 rounds = 0;
-	while (H) {
-		n_tasks.zero(ex, 1);
-		continuation_collect_fn cc = {tables.ptr(), K, heavy.ptr(), item_frag.ptr(), mism.ptr(), tasks.ptr(), n_tasks.ptr()};
-		for_each(ex, K, cc);
-		u32 Q = 0; n_tasks.download(ex, &Q, 1);
-		if (Q == 0) break;
-		spawned += Q; ++rounds;
-		for (u32 done = 0; done < Q; ) {
-			const u32 batch = std::min<u32>(Q - done, 0x80000000u / mismap_task_lanes);
-			mismap_task_fn mt = {items, tasks.ptr() + done, mismap_task_lanes, mismap_spawn_budget, tables.ptr(), K, overflow.ptr()};
-			for_each_occ<4>(ex, batch * mismap_task_lanes, mt);
+	timings.mismapper_heavy_items = H; timings.mismapper_table_slots = K;
+	u64 spawned = 0; u32 rounds = 0, overflows = 0;
+	dbuf<u32> n_tasks(1), overflow(1), n_redo(1);
+	for (u32 n = H; n; ) { // attempts: the items of this one are heavy[0, n)
+		dbuf<continuation_slot> tables((size_t) K + 1); dbuf<realign_task> tasks((size_t) K + 1); dbuf<u8> incomplete(n);
+		overflow.zero(ex, 1); incomplete.zero(ex, n);
+		continuation_init_fn ci = {tables.ptr()}; for_each(ex, K, ci);
+		const continuation_registry reg = {tables.ptr(), K, overflow.ptr(), incomplete.ptr()};
+		for (u32 done = 0; done < n; ) { // launches of at most 2^31 threads
+			const u32 batch = std::min<u32>(n - done, 0x80000000u / mismap_lanes);
+			mismap_heavy_fn mh = {items, heavy.ptr(), mismap_lanes, done, reg};
+			for_each_occ<4>(ex, batch * mismap_lanes, mh);
 			done += batch;
 		}
+		for (;;) {
+			n_tasks.zero(ex, 1);
+			continuation_collect_fn cc = {tables.ptr(), K, heavy.ptr(), item_frag.ptr(), mism.ptr(), tasks.ptr(), n_tasks.ptr()};
+			for_each(ex, K, cc);
+			u32 Q = 0; n_tasks.download(ex, &Q, 1);
+			if (Q == 0) break;
+			spawned += Q; ++rounds;
+			for (u32 done = 0; done < Q; ) {
+				const u32 batch = std::min<u32>(Q - done, 0x80000000u / mismap_task_lanes);
+				mismap_task_fn mt = {items, tasks.ptr() + done, mismap_task_lanes, reg};
+				for_each_occ<4>(ex, batch * mismap_task_lanes, mt);
+				done += batch;
+			}
+		}
+		u32 o = 0; overflow.download(ex, &o, 1); overflows += o;
+		if (o == 0) break;
+		// a registration did not fit: its continuation was dropped, so the undecided items it belonged to are re-aligned again with a larger table
+		dbuf<u32> redo(n); n_redo.zero(ex, 1);
+		incomplete_collect_fn ic = {incomplete.ptr(), heavy.ptr(), item_frag.ptr(), mism.ptr(), redo.ptr(), n_redo.ptr()};
+		for_each(ex, n, ic);
+		n_redo.download(ex, &n, 1);
+		heavy.swap(redo);
+		u64 next = K; while (next < std::max<u64>(4 * (u64) K, (u64) n * 4096)) next <<= 1;
+		if (n && next > (1u << 31)) throw arb_error("the continuation registry of the re-alignment would exceed 2^31 slots");
+		K = (u32) next;
 	}
-	timings.mismapper_tasks = spawned; timings.mismapper_rounds = rounds;
-	{ u32 o = 0; overflow.download(ex, &o, 1); timings.mismapper_overflow = o; timings.mismapper_table_slots = K; }
+	timings.mismapper_tasks = spawned; timings.mismapper_rounds = rounds; timings.mismapper_overflow = overflows;
 	timings.mismappers_pass2_ms = t2.stop();
-	timings.mismapper_heavy_items = H;
 	mismap_ms_part = t_all.stop();
 	ex.sync();
 }

@@ -81,7 +81,7 @@ ARB_HD u32 nt16_comp(u32 code) { return (u32) (0xFEDCBA9176523480ull >> (4 * cod
 // 2-bit code of a base for the 8-mer index: T=0 G=1 C=2, anything else 3 (filter_mismappers.cpp:33-45); table indexed by the nt16 code
 ARB_HD u32 nt16_base2(u32 code) { return 0xFFFCFDEFu >> (2 * code) & 3u; }
 
-// Everything one re-alignment keeps fixed across its recursion levels. realign() copies what it needs into registers on entry.
+// Everything one re-alignment keeps fixed across the searches of a (segment, gene, strand): the top-level search and its continuations.
 struct realign_env {
 	const u8* seq; u32 off, len; bool rc;        // the read slice
 	const i32* pos; const u32* bucket;           // k-mer hits and the 65,536 bucket offsets of the window's contig
@@ -106,32 +106,34 @@ ARB_HD bool env_ref_equals(const u32* g4, const char* ref, i32 g, u32 code) {
 	return g4 ? (g4[(u32) g >> 3] >> (28 - 4 * ((u32) g & 7)) & 15u) == code : ref[g] == nt16_char(code);
 }
 
-// Work control of one re-alignment. The reference's align() is a pure "does ANY placement reach min_score" search: the outcome is the OR over all
-// (read position, k-mer hit) pairs and over the recursive continuations, so the pairs may be visited in any order and by any number of threads.
-//  * budget: a `limited` search gives up after `budget` steps (the bounded attempt at a continuation before it is registered, spawn_budget);
-//  * lanes/lane/counter: the cooperative passes deal the top-level hits round-robin to `lanes` threads of the same item;
+// Work control of pass 2 and the task rounds. The reference's align() is a pure "does ANY placement reach min_score" search: the outcome is the OR over all
+// (read position, k-mer hit) pairs and over the continuations they start (at a splice site, at the first mismatch), so the pairs may be visited in any order
+// and by any number of threads.
+//  * lanes/lane/counter: `lanes` threads of the same search deal its hits round-robin (realign_search);
 //  * stop: set as soon as any lane (or any other item of the same fragment) found a placement.
-//  * table: in the cooperative passes a continuation (the recursive call at a splice site or at the first mismatch) is not run by the thread that meets
-//    it. It is REGISTERED in a hash table under (item, segment, gene, strand, score, read position, deletions left) with the smallest lower
-//    bound requested so far, and the caller goes on as if it had failed (valid: the answer is an OR). After the pass, every entry whose bound went down
-//    becomes one task; a group of lanes deals that task's hits and registers what IT cannot finish. A continuation only looks at hits at or above its
-//    bound, so the entry with the smallest bound answers for all the others: a read in a tandem repeat reaches the same (score, read position) from
-//    thousands of hits, and that is one task instead of thousands of identical searches.
+//  * table: a continuation is not run by the thread that meets it. It is REGISTERED in a hash table under (item, segment, gene, strand, score, read position,
+//    deletions left) with the smallest lower bound requested so far, and the caller goes on as if it had failed (valid: the answer is an OR). After the pass,
+//    every entry whose bound went down becomes one task; a group of lanes deals that task's hits and registers the continuations IT meets. A continuation
+//    only looks at hits at or above its bound, so the entry with the smallest bound answers for all the others: a read in a tandem repeat reaches the same
+//    (score, read position) from thousands of hits, and that is one task instead of thousands of identical searches. A registration that finds no room
+//    drops the continuation and marks the item incomplete: the driver re-runs the incomplete items with a larger table.
 //  * memo: a continuation is a pure function of (score, read position, deletions left, lower bound of the hits) and it only ever looks at hits at or
 //    above the lower bound. Once it has failed for a bound g it fails for every bound >= g. In a tandem repeat thousands of hits reach the same
-//    (score, read position) with ascending bounds: the first one pays, the others are answered from a small per-thread table.
+//    (score, read position) with ascending bounds: the first one registers, the others are answered from a small per-thread table without the atomics.
 struct realign_task { u32 item; u16 gene_k; u8 segment, rc; i32 score, read_pos, gene_pos, max_deletions; u32 item_slot; };
 struct continuation_slot { u64 key; i32 want /* smallest lower bound requested */, done /* bound already turned into a task */; };
-// key of a continuation: cooperative item (24 bits) | segment | strand | deletions left (2) | gene of the segment (10) | score + 512 (10) | read position (9); never 0
-ARB_HD bool continuation_key(const realign_task& t, u64& key) {
-	if (t.item_slot >= (1u << 24) || t.gene_k >= 1024 || t.score < -512 || t.score > 511 || t.read_pos < 0 || t.read_pos > 511 || t.max_deletions < 0 || t.max_deletions > 3) return false;
-	key = 1ull << 63 | (u64) t.item_slot << 33 | (u64) t.segment << 32 | (u64) t.rc << 31 | (u64) (u32) t.max_deletions << 29 | (u64) t.gene_k << 19 | (u64) (u32) (t.score + 512) << 9 | (u64) (u32) t.read_pos;
-	return true;
+// key of a continuation, never 0: cooperative item (24 bits) | segment | strand | deletions left (2) | gene of the segment (16) | score + 512 (10) | read
+// position (9). Every field fits: fewer than 2^24 items are re-aligned cooperatively, genes_cnt is a u16, and realign_can_start keeps the continuations of a
+// read under 300 bases within scores -316 .. 300 and read positions below 300.
+ARB_HD u64 continuation_key(const realign_task& t) {
+	return 1ull << 63 | (u64) t.item_slot << 39 | (u64) t.segment << 38 | (u64) t.rc << 37 | (u64) (u32) t.max_deletions << 35 | (u64) t.gene_k << 19 | (u64) (u32) (t.score + 512) << 9 | (u64) (u32) t.read_pos;
 }
 ARB_HD void continuation_unpack(u64 key, realign_task& t) {
-	t.item_slot = (u32) (key >> 33) & 0xFFFFFFu; t.segment = (u8) (key >> 32 & 1); t.rc = (u8) (key >> 31 & 1); t.max_deletions = (i32) (key >> 29 & 3); t.gene_k = (u16) (key >> 19 & 1023);
+	t.item_slot = (u32) (key >> 39) & 0xFFFFFFu; t.segment = (u8) (key >> 38 & 1); t.rc = (u8) (key >> 37 & 1); t.max_deletions = (i32) (key >> 35 & 3); t.gene_k = (u16) (key >> 19 & 0xFFFF);
 	t.score = (i32) (key >> 9 & 1023) - 512; t.read_pos = (i32) (key & 511);
 }
+// the registry of one attempt at the cooperative items: table_slots is a power of two; incomplete (per item slot) = a registration of the item did not fit
+struct continuation_registry { continuation_slot* table; u32 table_slots; u32* overflow /* registrations that did not fit */; u8* incomplete; };
 struct realign_memo { i32 score, read_pos, max_deletions, fail_from; };
 struct realign_ctl {
 	enum { MEMO_SLOTS = 16 };
@@ -146,113 +148,29 @@ struct realign_ctl {
 		const u32 slot = memo_n < MEMO_SLOTS ? memo_n++ : (memo_next++ % MEMO_SLOTS);
 		memo[slot].score = score; memo[slot].read_pos = read_pos; memo[slot].max_deletions = max_deletions; memo[slot].fail_from = gene_pos;
 	}
-	int budget; bool limited;
 	u32 lanes, lane, counter;
 	const volatile u8* stop;
-	int spawn_budget; continuation_slot* table; u32 table_slots; u32* overflow /* registrations that did not fit */; realign_task proto; // table: the item's registry; proto: item / segment / gene / strand of the running alignment
-	ARB_HD bool spawn(int score, int read_pos, int gene_pos, int max_deletions) { // registers the continuation; false if it cannot be (the caller then runs it itself)
+	continuation_registry reg; realign_task proto; // proto: item / segment / gene / strand of the running search
+	ARB_HD void spawn(int score, int read_pos, int gene_pos, int max_deletions) { // registers the continuation, or drops it and marks the item incomplete
 		realign_task t = proto; t.score = score; t.read_pos = read_pos; t.max_deletions = max_deletions;
-		u64 key;
-		if (!continuation_key(t, key)) return false;
+		const u64 key = continuation_key(t);
 		u64 h = key * 0x9E3779B97F4A7C15ULL; h ^= h >> 29;
-		for (u32 probe = 0; probe < 256; ++probe) { // table_slots is a power of two
-			continuation_slot& s = table[(h + probe) & (table_slots - 1)];
+		for (u32 probe = 0; probe < 256; ++probe) {
+			continuation_slot& s = reg.table[(h + probe) & (reg.table_slots - 1)];
 			const u64 seen = atomic_cas_u64(&s.key, 0, key);
-			if (seen == 0 || seen == key) { atomic_min_i32(&s.want, gene_pos); return true; }
+			if (seen == 0 || seen == key) { atomic_min_i32(&s.want, gene_pos); return; }
 		}
-		if (overflow) atomic_add_u32(overflow, 1);
-		return false;
+		atomic_add_u32(reg.overflow, 1);
+		reg.incomplete[proto.item_slot] = 1;
+	}
+	// the continuation sink of realign_extend
+	ARB_HD void operator()(int score, int read_pos, int gene_pos, int max_deletions) {
+		if (known_to_fail(score, read_pos, max_deletions, gene_pos)) return; // an identical continuation with a lower or equal bound is registered already
+		spawn(score, read_pos, gene_pos, max_deletions);
+		remember_failure(score, read_pos, max_deletions, gene_pos);
 	}
 };
-ARB_HD realign_ctl unlimited_ctl() { realign_ctl c; c.forget(); c.budget = 0; c.limited = false; c.lanes = 1; c.lane = 0; c.counter = 0; c.stop = 0; c.spawn_budget = 0; c.table = 0; c.table_slots = 0; c.overflow = 0; return c; }
-
-// seed-and-extend re-alignment (filter_mismappers.cpp:86-187): true as soon as a placement reaches min_score
-ARB_HD_RECURSIVE bool realign(int score, int read_pos, int gene_pos, int max_deletions, const realign_env& env, realign_ctl& ctl, bool top) {
-	const u8* const seq = env.seq; const u32 off = env.off; const bool rc = env.rc; const int len = (int) env.len;
-	const i32* const pos = env.pos; const u32* const bucket = env.bucket;
-	const i32 wstart = env.wstart, wend = env.wend; const int min_score = env.min_score;
-	const u32* const g4 = env.g4; const char* const ref = env.ref;
-	const bool limited = ctl.limited;
-	int budget = ctl.budget; // spent locally, written back on every way out
-	#define REALIGN_RETURN(x) do { ctl.budget = budget; return (x); } while (0)
-	#define REALIGN_CONTINUATION(sc, rp, gp, md) { \
-		if (ctl.known_to_fail(sc, rp, md, gp)) { /* an identical continuation with a lower or equal bound already failed (or is queued as a task) */ } \
-		else if (top && ctl.table) { /* cooperative passes: optional bounded attempt, then the item's registry */ \
-			bool found = false, undecided = true; \
-			if (ctl.spawn_budget > 0) { \
-				const bool was_limited = ctl.limited; ctl.limited = true; ctl.budget = ctl.spawn_budget; \
-				found = realign(sc, rp, gp, md, env, ctl, false); \
-				undecided = !found && ctl.budget < 0; ctl.limited = was_limited; \
-			} \
-			if (!found && undecided && !ctl.spawn(sc, rp, gp, md)) { ctl.budget = 0; found = realign(sc, rp, gp, md, env, ctl, false); } \
-			if (found) return true; \
-			ctl.remember_failure(sc, rp, md, gp); \
-		} else { \
-			ctl.budget = budget; \
-			if (realign(sc, rp, gp, md, env, ctl, false)) return true; \
-			budget = ctl.budget; \
-			if (!(limited && budget < 0)) ctl.remember_failure(sc, rp, md, gp); \
-		} }
-	if (!(read_pos + 8 < len && read_pos + min_score <= len + score + 16)) return false;
-	u32 km = 0;
-	for (u32 b = 0; b < 8; ++b) km = km << 2 | nt16_base2(env_code(seq, off, (u32) len, rc, (u32) read_pos + b));
-	int skipped = 0;
-	for (;;) {
-		const u32 lo = bucket[km], hi = bucket[km + 1];
-		if (lo != hi) {
-			u32 h = env_first_hit(env, km, lo, hi, gene_pos), step = 1;
-			if (top && ctl.lanes > 1) { // deal this position's hits to the lanes, continuing the round-robin of the previous positions
-				if (ctl.stop && *ctl.stop) REALIGN_RETURN(false);
-				const u32 n_hits = lower_bound_i32(pos, h, hi, wend) - h;
-				h += (ctl.lane + ctl.lanes - ctl.counter % ctl.lanes) % ctl.lanes; step = ctl.lanes;
-				ctl.counter += n_hits;
-			}
-			const bool leading = read_pos == skipped; // every base so far was skipped: no penalty for them (local alignment start)
-			for (; h < hi; h += step) {
-				const int hit = pos[h];
-				if (hit >= wend) break;
-				if (limited && --budget < 0) REALIGN_RETURN(false);
-				int ext = score + 8;
-				if (leading) ext += skipped;
-				if (ext >= min_score) REALIGN_RETURN(true);
-				{ // extend to the left over the skipped bases, one mismatch allowed
-					int r = read_pos - 1, g = hit - 1; u32 mm = 0;
-					while (r >= read_pos - skipped && g >= wstart) {
-						if (env_ref_equals(g4, ref, g, env_code(seq, off, (u32) len, rc, (u32) r))) { ext += leading ? 1 : 2; if (ext >= min_score) REALIGN_RETURN(true); }
-						else if (++mm > 1) break;
-						--r; --g;
-					}
-				}
-				{ // extend to the right; try a spliced continuation at splice sites and one deletion at the first mismatch
-					int r = read_pos + 8, g = hit + 8; u32 mm = 0, consecutive = 0;
-					u32 ss = lower_bound_i32(env.splice, 0, env.n_splice, g - 1);
-					i32 next_site = ss < env.n_splice ? env.splice[ss] : 0x7fffffff;
-					while (r < len && g <= wend) {
-						if (limited && --budget < 0) REALIGN_RETURN(false);
-						if (g - 1 >= next_site) {
-							if (g - 1 > next_site) { ++ss; next_site = ss < env.n_splice ? env.splice[ss] : 0x7fffffff; }
-							if (g - 1 == next_site) REALIGN_CONTINUATION(ext, r, g, max_deletions)
-						}
-						if (env_ref_equals(g4, ref, g, env_code(seq, off, (u32) len, rc, (u32) r))) { ++ext; if (ext >= min_score) REALIGN_RETURN(true); consecutive = 0; }
-						else {
-							if (++mm == 1 && max_deletions > 0 && len >= 30) REALIGN_CONTINUATION(ext, r, g, max_deletions - 1)
-							--ext;
-							if (++consecutive >= 4) break;
-						}
-						++r; ++g;
-					}
-				}
-			}
-		}
-		// next read position
-		if (!(read_pos + 9 < len && read_pos + 1 + min_score <= len + score - 1 + 16)) break;
-		km = (km << 2 | nt16_base2(env_code(seq, off, (u32) len, rc, (u32) read_pos + 8))) & 0xffffu;
-		++read_pos; --score; ++skipped;
-	}
-	REALIGN_RETURN(false);
-	#undef REALIGN_CONTINUATION
-	#undef REALIGN_RETURN
-}
+ARB_HD realign_ctl registry_ctl(u32 lanes, u32 lane, const u8* stop, const continuation_registry& reg) { realign_ctl c; c.forget(); c.lanes = lanes; c.lane = lane; c.counter = 0; c.stop = stop; c.reg = reg; return c; }
 
 struct gene_splice_view { const u32* off; const i32* sites; }; // per gene: sorted downstream splice sites (filter_mismappers.cpp:16-31)
 
@@ -283,19 +201,6 @@ ARB_HD bool segment_env(const realign_segment& s, u32 k, int max_mate_gap, const
 	env.min_score = s.min_score();
 	env.g4 = an.assembly4 ? an.assembly4 + an.contig_seq_off[contig] / 8 : 0; env.ref = an.assembly + an.contig_seq_off[contig];
 	return true;
-}
-ARB_HD bool realign_both_strands(const realign_segment& s, u32 segment, int max_mate_gap, const annot_view& an, const kmer_index_view& ix, const gene_splice_view& sp, realign_ctl& ctl) {
-	if (s.read.len >= 300) return false;
-	for (u32 k = 0; k < s.n_genes; ++k) {
-		realign_env env;
-		if (!segment_env(s, k, max_mate_gap, an, ix, sp, env)) continue;
-		ctl.proto.segment = (u8) segment; ctl.proto.gene_k = (u16) k;
-		ctl.proto.rc = 0; ctl.forget();
-		if (realign(0, 0, env.wstart, 1, env, ctl, true)) return true;
-		env.rc = !s.read.rc; ctl.proto.rc = 1; ctl.forget();
-		if (realign(0, 0, env.wstart, 1, env, ctl, true)) return true;
-	}
-	return false;
 }
 
 struct mismap_params { i32 max_mate_gap; float max_mismapper_fraction; };
@@ -339,19 +244,14 @@ struct mismap_items {
 		}
 		return s;
 	}
-	ARB_HD bool evaluate(u32 j, realign_ctl& ctl) const { // pass 2: pass 1 has tried the linear extension
-		ctl.proto.item = j;
-		for (u32 x = 0; x < 2; ++x) if (realign_both_strands(segment(j, x), x, p.max_mate_gap, an, ix, sp, ctl)) return true;
-		return false;
-	}
 };
 
-// ---- pass 1: a GROUP of lanes per item, without recursion ---------------------------------------------------------------------------------------------
+// ---- pass 1: a GROUP of lanes per item, continuations on a worklist -----------------------------------------------------------------------------------
 // The search is an OR over (read position, k-mer hit) pairs and over the continuations they start (a continuation = the same search from a later read
 // position with a lower bound on the hits). Read positions are independent of each other -- score and skipped bases at position p follow from p alone -- so
 // the lanes of a group take the positions of a search in turn, and a continuation is not called but pushed on the group's small worklist (shared memory)
-// and searched by the whole group later. No device recursion, no per-thread memo in local memory; the order of evaluation differs from the reference's,
-// the result (an OR) does not. An item that overflows the worklist or the step budget goes to the cooperative pass 2.
+// and searched by the whole group later. No per-thread memo in local memory; the order of evaluation differs from the reference's, the result (an OR) does
+// not. An item that overflows the worklist or the step budget goes to the cooperative pass 2.
 struct realign_work { i32 gene_pos; i16 score; u16 read_pos; u16 gene_k; u8 segment, rc_deletions /* bit 7 strand, bits 0..6 deletions left */; };
 struct realign_worklist { realign_work* tasks; u32* top; u32 capacity; };
 ARB_HD u32 worklist_fetch_add(u32* p, u32 v) {
@@ -362,13 +262,15 @@ ARB_HD u32 worklist_fetch_add(u32* p, u32 v) {
 #endif
 }
 ARB_HD bool realign_can_start(int score, int read_pos, int len, int min_score) { return read_pos + 8 < len && read_pos + min_score <= len + score + 16; } // filter_mismappers.cpp:90-94
-ARB_HD void worklist_push(const realign_worklist& wl, const realign_work& current, int score, int read_pos, int gene_pos, int max_deletions, int len, int min_score) {
-	if (!realign_can_start(score, read_pos, len, min_score)) return; // the continuation would return at once
-	const u32 slot = worklist_fetch_add(wl.top, 1);
-	if (slot >= wl.capacity) return; // noticed by the group when it reads `top` next: the item goes to pass 2
-	realign_work t = current; t.score = (i16) score; t.read_pos = (u16) read_pos; t.gene_pos = gene_pos; t.rc_deletions = (u8) ((current.rc_deletions & 0x80u) | (u32) max_deletions);
-	wl.tasks[slot] = t;
-}
+struct worklist_push { // the continuation sink of pass 1: a continuation of `current` goes on the group's worklist
+	const realign_worklist& wl; const realign_work& current;
+	ARB_HD void operator()(int score, int read_pos, int gene_pos, int max_deletions) const {
+		const u32 slot = worklist_fetch_add(wl.top, 1);
+		if (slot >= wl.capacity) return; // noticed by the group when it reads `top` next: the item goes to pass 2
+		realign_work t = current; t.score = (i16) score; t.read_pos = (u16) read_pos; t.gene_pos = gene_pos; t.rc_deletions = (u8) ((current.rc_deletions & 0x80u) | (u32) max_deletions);
+		wl.tasks[slot] = t;
+	}
+};
 // 8-mer (2 bits per base) of the read slice at position r, on the strand of the search
 ARB_HD u32 env_kmer(const realign_env& env, u32 r) {
 	if (!env.rc) return nt16_dense2(nt16_window(env.seq, 0x7fffffffu, (i32) (env.off + r)));
@@ -376,9 +278,6 @@ ARB_HD u32 env_kmer(const realign_env& env, u32 r) {
 	// and complements A/C/G/T/N; every other code keeps more than one bit and maps to 3 like the character it stands for
 	return nt16_dense2(brev32(nt16_window(env.seq, 0x7fffffffu, (i32) (env.off + env.len - 8 - r))));
 }
-// One search (top level or continuation) by the lanes of a group: the lanes take the read positions in turn (score and skipped bases at a position follow
-// from the position alone); a lane looks up its position's 8-mer, finds the first hit at or after the lower bound through the block table and extends
-// every hit inside the window. Returns REALIGN_FOUND on the lane that reached min_score (the caller combines the lanes).
 enum { REALIGN_UNDECIDED_NO = 0, REALIGN_FOUND = 1, REALIGN_EXHAUSTED = 2 };
 // Eight bases of the read slice (on the strand of the search, from base r0) against eight reference bases from g0, in one XOR of packed words:
 // bit 28 - 4j of `differs` is set where base r0 + j differs from reference base g0 + j. false = this stretch has to be compared base by base (no packed
@@ -402,13 +301,16 @@ ARB_HD bool env_differs8(const realign_env& env, int r0, int g0, int first, int 
 	differs = (x | x >> 1 | x >> 2 | x >> 3) & 0x11111111u;
 	return true;
 }
-ARB_HD bool realign_extend(const realign_env& env, const realign_work& task, const realign_worklist& wl, int read_pos, int hit, u32& steps) {
+// The extension of one (read position, k-mer hit) pair of the search that starts at (score0, read_pos0, max_deletions) (filter_mismappers.cpp:86-187), in every
+// pass: true as soon as the placement reaches min_score. A continuation it meets -- at a splice site, and one deletion at the first mismatch -- is not run
+// here but handed to `sink(score, read_pos, gene_pos, max_deletions)` unless it would stop at once: pass 1 pushes it on the group's worklist, pass 2 and the
+// task rounds register it (realign_ctl).
+template <class Sink> ARB_HD bool realign_extend(const realign_env& env, int score0, int read_pos0, int max_deletions, int read_pos, int hit, Sink& sink, u32& steps) {
 	const u8* const seq = env.seq; const u32 off = env.off; const bool rc = env.rc; const int len = (int) env.len;
 	const i32 wstart = env.wstart, wend = env.wend; const int min_score = env.min_score;
 	const u32* const g4 = env.g4; const char* const ref = env.ref;
-	const int read_pos0 = task.read_pos, max_deletions = task.rc_deletions & 0x7f;
 	const bool leading = read_pos0 == 0; // every base before the seed was skipped: no penalty for them (local alignment start)
-	const int skipped = read_pos - read_pos0, score = (int) task.score - skipped;
+	const int skipped = read_pos - read_pos0, score = score0 - skipped;
 	++steps;
 	int ext = score + 8;
 	if (leading) ext += skipped;
@@ -433,7 +335,7 @@ ARB_HD bool realign_extend(const realign_env& env, const realign_work& task, con
 			}
 		}
 	}
-	{ // extend to the right; a spliced continuation at splice sites and one deletion at the first mismatch go to the worklist
+	{ // extend to the right; a spliced continuation at splice sites and one deletion at the first mismatch go to the sink
 		int r = read_pos + 8, gp = hit + 8; u32 mm = 0, consecutive = 0;
 		u32 ss = lower_bound_i32(env.splice, 0, env.n_splice, gp - 1);
 		i32 next_site = ss < env.n_splice ? env.splice[ss] : 0x7fffffff;
@@ -445,11 +347,11 @@ ARB_HD bool realign_extend(const realign_env& env, const realign_work& task, con
 				++steps;
 				if (gp - 1 >= next_site) {
 					if (gp - 1 > next_site) { ++ss; next_site = ss < env.n_splice ? env.splice[ss] : 0x7fffffff; }
-					if (gp - 1 == next_site) worklist_push(wl, task, ext, r, gp, max_deletions, len, min_score);
+					if (gp - 1 == next_site && realign_can_start(ext, r, len, min_score)) sink(ext, r, gp, max_deletions);
 				}
 				if (!(differs >> (28 - 4 * j) & 1u)) { ++ext; if (ext >= min_score) return true; consecutive = 0; }
 				else {
-					if (++mm == 1 && max_deletions > 0 && len >= 30) worklist_push(wl, task, ext, r, gp, max_deletions - 1, len, min_score);
+					if (++mm == 1 && max_deletions > 0 && len >= 30 && realign_can_start(ext, r, len, min_score)) sink(ext, r, gp, max_deletions - 1);
 					--ext;
 					if (++consecutive >= 4) return false;
 				}
@@ -458,11 +360,15 @@ ARB_HD bool realign_extend(const realign_env& env, const realign_work& task, con
 	}
 	return false;
 }
+// One search (top level or continuation) by the lanes of a group: the lanes take the read positions in turn (score and skipped bases at a position follow
+// from the position alone); a lane looks up its position's 8-mer, finds the first hit at or after the lower bound through the block table and extends
+// every hit inside the window. Returns REALIGN_FOUND on the lane that reached min_score (the caller combines the lanes).
 ARB_HD u32 realign_group(const lane_group& g, const realign_env& env, const realign_work& task, const realign_worklist& wl, u32& steps, u32& hits) {
 	const int len = (int) env.len;
 	const i32* const pos = env.pos; const u32* const bucket = env.bucket;
 	const i32 wend = env.wend; const int min_score = env.min_score;
-	const int read_pos0 = task.read_pos, score0 = task.score, gene_pos = task.gene_pos;
+	const int read_pos0 = task.read_pos, score0 = task.score, gene_pos = task.gene_pos, max_deletions = task.rc_deletions & 0x7f;
+	worklist_push sink = {wl, task};
 	for (int read_pos = read_pos0 + (int) g.lane; ; read_pos += (int) g.lanes) {
 		if (!realign_can_start(score0 - (read_pos - read_pos0), read_pos, len, min_score)) return REALIGN_UNDECIDED_NO; // the valid positions are a prefix
 		const u32 km = env_kmer(env, (u32) read_pos);
@@ -472,9 +378,32 @@ ARB_HD u32 realign_group(const lane_group& g, const realign_env& env, const real
 			const int hit = pos[h];
 			if (hit >= wend) break;
 			++hits;
-			if (realign_extend(env, task, wl, read_pos, hit, steps)) return REALIGN_FOUND;
+			if (realign_extend(env, score0, read_pos0, max_deletions, read_pos, hit, sink, steps)) return REALIGN_FOUND;
 		}
 	}
+}
+// One search (top level or continuation) in pass 2 and the task rounds: every lane walks the read positions, and the hits of each position are dealt
+// round-robin to the `lanes` threads of the search, continuing the deal of the previous positions (ctl.counter) so that positions with few hits do not all
+// fall to the first lanes. Continuations go to the registry.
+ARB_HD bool realign_search(const realign_env& env, int score0, int read_pos0, int gene_pos, int max_deletions, realign_ctl& ctl) {
+	const i32* const pos = env.pos;
+	u32 steps = 0; // pass 1's budget; not counted here
+	for (int read_pos = read_pos0; realign_can_start(score0 - (read_pos - read_pos0), read_pos, (int) env.len, env.min_score); ++read_pos) {
+		const u32 km = env_kmer(env, (u32) read_pos);
+		const u32 lo = env.bucket[km], hi = env.bucket[km + 1];
+		if (lo == hi) continue;
+		if (*ctl.stop) return false;
+		u32 h = env_first_hit(env, km, lo, hi, gene_pos);
+		const u32 n_hits = lower_bound_i32(pos, h, hi, env.wend) - h;
+		h += (ctl.lane + ctl.lanes - ctl.counter % ctl.lanes) % ctl.lanes;
+		ctl.counter += n_hits;
+		for (; h < hi; h += ctl.lanes) {
+			const int hit = pos[h];
+			if (hit >= env.wend) break;
+			if (realign_extend(env, score0, read_pos0, max_deletions, read_pos, hit, ctl, steps)) return true;
+		}
+	}
+	return false;
 }
 
 // filter_mismappers.cpp:247-270: can the clipped segment simply be extended along the reference? The lanes of the group share the clipped bases.
@@ -566,15 +495,27 @@ struct mismap_item_group_fn {
 		else if (verdict == REALIGN_EXHAUSTED) heavy[atomic_add_u32(n_heavy, 1)] = j;
 	}
 };
-// pass 2: `lanes` threads per queued item share the top-level k-mer hits; continuations go to the item's registry
+// pass 2: `lanes` threads per queued item share the top-level k-mer hits of both sequences of the item against every gene of the other breakpoint, both
+// strands (filter_mismappers.cpp:189-230, :296-333; pass 1 has tried the linear extension); continuations go to the registry
 struct mismap_heavy_fn {
-	mismap_items it; const u32* heavy; u32 lanes; int spawn_budget; continuation_slot* tables; u32 table_slots; u32 first_slot; u32* overflow;
+	mismap_items it; const u32* heavy; u32 lanes; u32 first_slot; continuation_registry reg;
 	ARB_HD void operator()(u32 t) const {
 		const u32 slot = first_slot + t / lanes, j = heavy[slot], i = it.item_frag[j];
-		realign_ctl ctl = unlimited_ctl(); ctl.lanes = lanes; ctl.lane = t % lanes; ctl.stop = it.mismapper + i;
-		ctl.spawn_budget = spawn_budget; ctl.table = tables; ctl.table_slots = table_slots; ctl.overflow = overflow; ctl.proto.item_slot = slot;
+		realign_ctl ctl = registry_ctl(lanes, t % lanes, it.mismapper + i, reg); ctl.proto.item = j; ctl.proto.item_slot = slot;
 		if (*ctl.stop) return;
-		if (it.evaluate(j, ctl)) it.mismapper[i] = 1;
+		for (u32 x = 0; x < 2; ++x) {
+			const realign_segment s = it.segment(j, x);
+			if (s.read.len >= 300) continue;
+			for (u32 k = 0; k < s.n_genes; ++k) {
+				realign_env env;
+				if (!segment_env(s, k, it.p.max_mate_gap, it.an, it.ix, it.sp, env)) continue;
+				ctl.proto.segment = (u8) x; ctl.proto.gene_k = (u16) k;
+				for (u32 strand = 0; strand < 2; ++strand) {
+					env.rc = strand ? !s.read.rc : s.read.rc; ctl.proto.rc = (u8) strand; ctl.forget();
+					if (realign_search(env, 0, 0, env.wstart, 1, ctl)) { it.mismapper[i] = 1; return; }
+				}
+			}
+		}
 	}
 };
 struct continuation_init_fn { continuation_slot* tables; ARB_HD void operator()(u32 k) const { tables[k].key = 0; tables[k].want = 0x7fffffff; tables[k].done = 0x7fffffff; } };
@@ -594,19 +535,23 @@ struct continuation_collect_fn {
 };
 // task rounds: `lanes` threads per registered continuation
 struct mismap_task_fn {
-	mismap_items it; const realign_task* tasks; u32 lanes; int spawn_budget; continuation_slot* tables; u32 table_slots; u32* overflow;
+	mismap_items it; const realign_task* tasks; u32 lanes; continuation_registry reg;
 	ARB_HD void operator()(u32 t) const {
 		const realign_task task = tasks[t / lanes];
 		const u32 i = it.item_frag[task.item];
-		realign_ctl ctl = unlimited_ctl(); ctl.lanes = lanes; ctl.lane = t % lanes; ctl.stop = it.mismapper + i;
-		ctl.spawn_budget = spawn_budget; ctl.table = tables; ctl.table_slots = table_slots; ctl.overflow = overflow; ctl.proto = task;
+		realign_ctl ctl = registry_ctl(lanes, t % lanes, it.mismapper + i, reg); ctl.proto = task;
 		if (*ctl.stop) return;
 		const realign_segment s = it.segment(task.item, task.segment);
 		realign_env env;
 		if (!segment_env(s, task.gene_k, it.p.max_mate_gap, it.an, it.ix, it.sp, env)) return;
 		if (task.rc) env.rc = !s.read.rc;
-		if (realign(task.score, task.read_pos, task.gene_pos, task.max_deletions, env, ctl, true)) it.mismapper[i] = 1;
+		if (realign_search(env, task.score, task.read_pos, task.gene_pos, task.max_deletions, ctl)) it.mismapper[i] = 1;
 	}
+};
+// after the rounds: the items a registration failed for whose fragment is still undecided, to be re-aligned again with a larger registry
+struct incomplete_collect_fn {
+	const u8* incomplete; const u32* heavy; const u32* item_frag; const u8* mismapper; u32* redo; u32* n_redo;
+	ARB_HD void operator()(u32 slot) const { if (incomplete[slot] && !mismapper[item_frag[heavy[slot]]]) redo[append_slot(n_redo)] = heavy[slot]; }
 };
 
 struct mismap_apply_fn { const u8* mismapper; u8* filter; ARB_HD void operator()(u32 i) const { if (mismapper[i] && filter[i] == F_none) filter[i] = F_mismappers; } };

@@ -171,7 +171,7 @@ template <class F> void for_each(const exec_ctx& ex, u32 n, const F& f) {
 	ARB_CUDA_CHECK(cudaGetLastError());
 	++stats().kernels;
 }
-// same, with a register cap: at least MIN_BLOCKS resident 256-thread blocks per SM (the recursive re-alignment kernels trade spills for occupancy)
+// same, with a register cap: at least MIN_BLOCKS resident 256-thread blocks per SM (the cooperative re-alignment kernels, whose many threads per item want occupancy)
 template <int MIN_BLOCKS, class F> __global__ void __launch_bounds__(256, MIN_BLOCKS) k_for_each_occ(u32 n, F f) {
 	u32 i = blockIdx.x * 256u + threadIdx.x;
 	if (i < n) f(i);

@@ -79,20 +79,23 @@ def test_events_hostsim_mismapper_heavy(worlds, hostsim_lib):
 
 def test_events_hostsim_cooperative_realignment(worlds, hostsim_lib, monkeypatch):
     """A tiny step budget pushes almost every (candidate, read) pair through the cooperative second pass; labels must not change."""
-    monkeypatch.setenv("ARB_MISMAP_BUDGET", "24"); monkeypatch.setenv("ARB_MISMAP_LANES", "7")
-    monkeypatch.setenv("ARB_MISMAP_SPAWN", "6"); monkeypatch.setenv("ARB_MISMAP_TASK_LANES", "3")
+    monkeypatch.setenv("ARB_MISMAP_BUDGET", "24"); monkeypatch.setenv("ARB_MISMAP_LANES", "7"); monkeypatch.setenv("ARB_MISMAP_TASK_LANES", "3")
     p = check_events(worlds.get("cfg5", **CFG5), hostsim_lib, keep=True)
     tm = p.context().timings(); p.close()
     assert tm.mismapper_heavy_items > 0.2 * tm.mismapper_items
     assert tm.mismapper_tasks > 1000 and tm.mismapper_rounds >= 2   # continuations of continuations were registered as well
 
 
-@pytest.mark.parametrize("spawn,table", [("0", "1048576"), ("0", "64"), ("5", "1")])
-def test_events_hostsim_continuation_registry(worlds, hostsim_lib, monkeypatch, spawn, table):
-    """No bounded attempts (every continuation is registered), and registries so small that most registrations fail over to the in-line search."""
+@pytest.mark.parametrize("table", ["1048576", "64", "1"])
+def test_events_hostsim_continuation_registry(worlds, hostsim_lib, monkeypatch, table):
+    """A registry large enough for every continuation, and first registries so small that registrations fail: the items they belong to are re-aligned again
+    with a larger one."""
     monkeypatch.setenv("ARB_MISMAP_BUDGET", "24"); monkeypatch.setenv("ARB_MISMAP_LANES", "5")
-    monkeypatch.setenv("ARB_MISMAP_SPAWN", spawn); monkeypatch.setenv("ARB_MISMAP_TASK_LANES", "4"); monkeypatch.setenv("ARB_MISMAP_TABLE_TOTAL", table)
-    check_events(worlds.get("cfg5", **CFG5), hostsim_lib)
+    monkeypatch.setenv("ARB_MISMAP_TASK_LANES", "4"); monkeypatch.setenv("ARB_MISMAP_TABLE_TOTAL", table)
+    p = check_events(worlds.get("cfg5", **CFG5), hostsim_lib, keep=True)
+    tm = p.context().timings(); p.close()
+    if int(table) <= 64:
+        assert tm.mismapper_overflow > 0
 
 
 @pytest.mark.parametrize("lanes", ["1", "7"])
@@ -115,10 +118,9 @@ def test_events_cuda_mismapper_heavy(worlds, cuda_lib):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("budget,lanes,spawn,task_lanes", [("16", "32", "4", "32"), ("200", "256", "0", "32"), ("0", "1", "0", "1"), ("64", "8", "16", "5")])
-def test_events_cuda_cooperative_realignment(worlds, cuda_lib, monkeypatch, budget, lanes, spawn, task_lanes):
-    monkeypatch.setenv("ARB_MISMAP_BUDGET", budget); monkeypatch.setenv("ARB_MISMAP_LANES", lanes)
-    monkeypatch.setenv("ARB_MISMAP_SPAWN", spawn); monkeypatch.setenv("ARB_MISMAP_TASK_LANES", task_lanes)
+@pytest.mark.parametrize("budget,lanes,task_lanes", [("16", "32", "32"), ("200", "256", "32"), ("0", "1", "1"), ("64", "8", "5")])
+def test_events_cuda_cooperative_realignment(worlds, cuda_lib, monkeypatch, budget, lanes, task_lanes):
+    monkeypatch.setenv("ARB_MISMAP_BUDGET", budget); monkeypatch.setenv("ARB_MISMAP_LANES", lanes); monkeypatch.setenv("ARB_MISMAP_TASK_LANES", task_lanes)
     check_events(worlds.get("cfg5", **CFG5), cuda_lib)
 
 
