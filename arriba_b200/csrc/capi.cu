@@ -148,6 +148,7 @@ int arb_filter_mismappers_part(arb_ctx* ctx, int32_t max_mate_gap, int part, int
 int arb_filter_mismappers_finish(arb_ctx* ctx, uint64_t* n) { ARB_API_BEGIN(ctx) const uint64_t k = ctx->e.filter_mismappers_finish(); if (n) *n = k; ARB_API_END(ctx) }
 int arb_get_timings(arb_ctx* ctx, arb_timings* out) { ARB_API_BEGIN(ctx) *out = ctx->e.timings; ARB_API_END(ctx) }
 int arb_selftest_mismatch_counts(arb_ctx* ctx, uint32_t* out) { ARB_API_BEGIN(ctx) ctx->e.probe_mismatch_counts(out); ARB_API_END(ctx) } // tests only, not declared in the public header
+int arb_selftest_kmer_lookup(arb_ctx* ctx, const uint32_t* contig, const uint32_t* kmer, const int32_t* from, uint32_t n, uint32_t* out) { ARB_API_BEGIN(ctx) ctx->e.probe_kmer_lookup(contig, kmer, from, n, out); ARB_API_END(ctx) } // tests only, as above
 int arb_set_genomic_breakpoints(arb_ctx* ctx, uint32_t n, const uint16_t* c1, const uint16_t* c2, const uint8_t* d1, const uint8_t* d2, const int32_t* p1, const int32_t* p2) {
 	ARB_API_BEGIN(ctx) ctx->e.set_genomic_breakpoints(n, c1, c2, d1, d2, p1, p2); ARB_API_END(ctx)
 }

@@ -165,6 +165,7 @@ public:
 	void homolog_pairs(const u32* ga, const u32* gb, u32 n, u8* out);
 	u64 filter_mismappers(i32 max_mate_gap);
 	void probe_mismatch_counts(u32* out); // test hook (arb_selftest_mismatch_counts)
+	void probe_kmer_lookup(const u32* contig, const u32* kmer, const i32* from, u32 n, u32* out); // test hook (arb_selftest_kmer_lookup)
 	// genomic breakpoints from whole-genome sequencing (genomic.cu): sorted records + key table, the search writes cands.closest1/2
 	void set_genomic_breakpoints(u32 n, const u16* c1, const u16* c2, const u8* d1, const u8* d2, const i32* p1, const i32* p2);
 	u32 mark_genomic_support(i32 max_distance, i32 max_itd_length); void get_genomic_support(i32* closest1, i32* closest2);

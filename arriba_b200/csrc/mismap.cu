@@ -104,6 +104,19 @@ kmer_index_view engine::index_view() {
 	return ix;
 }
 
+void engine::probe_kmer_lookup(const u32* contig, const u32* kmer, const i32* from, u32 n, u32* out) {
+	if (n == 0) return;
+	for (u32 j = 0; j < n; ++j) {
+		if (contig[j] >= kmer_index_contigs || kmer[j] > 0xFFFFu) throw arb_error("arb_selftest_kmer_lookup: contig not indexed or 8-mer out of range");
+		if (from[j] > 0 && (u64) from[j] >= (u64) (contig[j] < annot.h_contig_len.size() ? annot.h_contig_len[contig[j]] : 0)) throw arb_error("arb_selftest_kmer_lookup: bound past the contig's end");
+	}
+	dbuf<u32> c, k, o((size_t) n * 6); dbuf<i32> f;
+	c.upload(ex, contig, n); k.upload(ex, kmer, n); f.upload(ex, from, n);
+	kmer_lookup_fn fn = {index_view(), c.ptr(), k.ptr(), f.ptr(), o.ptr()};
+	for_each(ex, n, fn);
+	o.download(ex, out, (size_t) n * 6);
+}
+
 void engine::homolog_pairs(const u32* ga, const u32* gb, u32 n, u8* out) {
 	if (n == 0) return;
 	dbuf<u32> a, b; dbuf<u8> o(n);

@@ -91,6 +91,11 @@ struct realign_env {
 	int min_score;
 	const u32* g4; const char* ref;              // reference of the contig: packed nt16 codes, or characters when g4 == 0
 };
+// the index part of the env: hits, bucket offsets and block table of one (indexed) contig
+ARB_HD void env_index(const kmer_index_view& ix, u32 contig, realign_env& env) {
+	env.pos = ix.pos; env.bucket = ix.bucket_off + (u64) contig * 65536;
+	env.block_first = ix.block_first + ((u64) ix.contig_block_base[contig] << 16); env.block_shift = ix.block_shift;
+}
 // first hit of the non-empty bucket [lo, hi) of `km` at or after gene_pos
 ARB_HD u32 env_first_hit(const realign_env& env, u32 km, u32 lo, u32 hi, i32 gene_pos) {
 	if (gene_pos <= 0) return lo;
@@ -195,13 +200,26 @@ ARB_HD bool segment_env(const realign_segment& s, u32 k, int max_mate_gap, const
 	if (s.same_contig && ((s.aln_start >= env.wstart && s.aln_start <= env.wend) || (s.aln_end >= env.wstart && s.aln_end <= env.wend))) return false;
 	if (contig >= ix.n_index_contigs) return false;
 	env.seq = s.read.nt16; env.off = s.read.off; env.len = s.read.len; env.rc = s.read.rc;
-	env.pos = ix.pos; env.bucket = ix.bucket_off + (u64) contig * 65536;
-	env.block_first = ix.block_first + ((u64) ix.contig_block_base[contig] << 16); env.block_shift = ix.block_shift;
+	env_index(ix, contig, env);
 	env.splice = sp.sites + sp.off[g]; env.n_splice = sp.off[g + 1] - sp.off[g];
 	env.min_score = s.min_score();
 	env.g4 = an.assembly4 ? an.assembly4 + an.contig_seq_off[contig] / 8 : 0; env.ref = an.assembly + an.contig_seq_off[contig];
 	return true;
 }
+
+// test hook (arb_selftest_kmer_lookup): per query (contig, 8-mer, lower bound) the bucket [lo, hi) and the first hit at or after the bound, found twice:
+// through kmer_index_view::first_at_or_after (gene homology) and through env_first_hit (re-alignment); out = lo, hi, hit, its position (~0 if none) x 2
+struct kmer_lookup_fn {
+	kmer_index_view ix; const u32* contig; const u32* kmer; const i32* from; u32* out;
+	ARB_HD void operator()(u32 j) const {
+		u32 lo, hi; ix.bucket(contig[j], kmer[j], lo, hi);
+		const u32 h1 = ix.first_at_or_after(contig[j], kmer[j], lo, hi, from[j]);
+		realign_env env; env_index(ix, contig[j], env);
+		const u32 h2 = lo == hi ? lo : env_first_hit(env, kmer[j], lo, hi, from[j]);
+		u32* o = out + 6 * (size_t) j;
+		o[0] = lo; o[1] = hi; o[2] = h1; o[3] = h1 < hi ? (u32) ix.pos[h1] : ~0u; o[4] = h2; o[5] = h2 < hi ? (u32) ix.pos[h2] : ~0u;
+	}
+};
 
 struct mismap_params { i32 max_mate_gap; float max_mismapper_fraction; };
 

@@ -128,7 +128,12 @@ def load(path=None):
                        ("arb_swaps_buffer", [_p(C.c_void_p), _p(C.c_uint64)]), ("arb_swaps_apply", []),
                        ("arb_filter_mismappers_part", [C.c_int32, C.c_int, C.c_int, _p(C.c_void_p), _p(C.c_uint64)]), ("arb_filter_mismappers_finish", [_p(C.c_uint64)]),
                        ("arb_set_genomic_breakpoints", [C.c_uint32, _p(C.c_uint16), _p(C.c_uint16), _p(C.c_uint8), _p(C.c_uint8), _p(C.c_int32), _p(C.c_int32)]),
-                       ("arb_mark_genomic_support", [C.c_int32, C.c_int32, _p(C.c_uint32)]), ("arb_get_genomic_support", [_p(C.c_int32), _p(C.c_int32)])]:
+                       ("arb_mark_genomic_support", [C.c_int32, C.c_int32, _p(C.c_uint32)]), ("arb_get_genomic_support", [_p(C.c_int32), _p(C.c_int32)]),
+                       ("arb_set_candidate_state", [_p(C.c_uint8), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_float)]),
+                       ("arb_set_candidate_lists", [_p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32)]),
+                       ("arb_set_splice_sites", [_p(C.c_uint32), _p(C.c_int32)]),
+                       ("arb_build_kmer_index", [_p(C.c_uint32), _p(C.c_int32), _p(C.c_int32), C.c_uint32, C.c_uint32, _p(C.c_uint64)]),
+                       ("arb_homolog_pairs", [_p(C.c_uint32), _p(C.c_uint32), C.c_uint32, _p(C.c_uint8)]), ("arb_filter_mismappers", [C.c_int32, _p(C.c_uint64)])]:
         fn = getattr(lib, name)
         fn.argtypes = [C.c_void_p] + args
         fn.restype = C.c_int
@@ -332,6 +337,46 @@ class Context:
         s = np.zeros(self.n_fragments, np.uint8)
         self._check(self.lib.arb_get_slot_swaps(self.h, ptr(s)))
         return s
+
+    # ---- candidate state, k-mer index, gene homology and re-alignment (filter_homologs, filter_mismappers)
+    def set_candidate_state(self, filter, split_reads1, split_reads2, discordant_mates, evalue):
+        """Per-candidate columns in candidate order, as arb_get_candidates returns them."""
+        cols = [np.ascontiguousarray(a, dt) for a, dt in ((filter, np.uint8), (split_reads1, np.uint32), (split_reads2, np.uint32), (discordant_mates, np.uint32), (evalue, np.float32))]
+        cols = [c if c.size else np.zeros(1, c.dtype) for c in cols]
+        self._check(self.lib.arb_set_candidate_state(self.h, *[ptr(c) for c in cols]))
+
+    def set_candidate_lists(self, list1_off, list1, list2_off, list2):
+        """Replaces the split-read lists (CSR: offsets n + 1, fragment indices) of the resident candidates."""
+        cols = [np.ascontiguousarray(a, np.uint32) for a in (list1_off, list1, list2_off, list2)]
+        cols = [c if c.size else np.zeros(1, np.uint32) for c in cols]
+        self._check(self.lib.arb_set_candidate_lists(self.h, *[ptr(c) for c in cols]))
+
+    def set_splice_sites(self, off, sites):
+        """Downstream splice sites per gene: off (n_genes + 1) into the sorted sites of each gene."""
+        off = np.ascontiguousarray(off, np.uint32); sites = np.ascontiguousarray(sites, np.int32)
+        self._check(self.lib.arb_set_splice_sites(self.h, ptr(off), ptr(sites if sites.size else np.zeros(1, np.int32))))
+
+    def build_kmer_index(self, contig, start, end, n_index_contigs):
+        """8-mer index over the intervals [start, end) of positions; returns the number of positions indexed."""
+        cols = [np.ascontiguousarray(a, dt) for a, dt in ((contig, np.uint32), (start, np.int32), (end, np.int32))]
+        n = cols[0].size
+        cols = [c if c.size else np.zeros(1, c.dtype) for c in cols]
+        k = C.c_uint64()
+        self._check(self.lib.arb_build_kmer_index(self.h, *[ptr(c) for c in cols], n, int(n_index_contigs), C.byref(k)))
+        return int(k.value)
+
+    def homolog_pairs(self, gene_a, gene_b):
+        """is_homolog(gene_a[j], gene_b[j]) for every j, at the context's max_homolog_identity."""
+        a = np.ascontiguousarray(gene_a, np.uint32); b = np.ascontiguousarray(gene_b, np.uint32)
+        out = np.zeros(max(a.size, 1), np.uint8)
+        self._check(self.lib.arb_homolog_pairs(self.h, ptr(a), ptr(b), a.size, ptr(out)))
+        return out[:a.size].astype(bool)
+
+    def filter_mismappers(self, max_mate_gap):
+        """Re-aligns the listed reads of the unfiltered candidates; returns the number of (candidate, fragment) items."""
+        n = C.c_uint64()
+        self._check(self.lib.arb_filter_mismappers(self.h, int(max_mate_gap), C.byref(n)))
+        return int(n.value)
 
 
 # ------------------------------------------------------------------------------------------- whole-run driver
