@@ -154,6 +154,13 @@ int arb_set_genomic_breakpoints(arb_ctx* ctx, uint32_t n, const uint16_t* c1, co
 }
 int arb_mark_genomic_support(arb_ctx* ctx, int32_t max_distance, int32_t max_itd_length, uint32_t* marked) { ARB_API_BEGIN(ctx) const uint32_t m = ctx->e.mark_genomic_support(max_distance, max_itd_length); if (marked) *marked = m; ARB_API_END(ctx) }
 int arb_get_genomic_support(arb_ctx* ctx, int32_t* closest1, int32_t* closest2) { ARB_API_BEGIN(ctx) ctx->e.get_genomic_support(closest1, closest2); ARB_API_END(ctx) }
+int arb_set_blacklist(arb_ctx* ctx, uint32_t n, const uint8_t* t1, const uint8_t* t2, const uint8_t* s1, const uint8_t* s2, const uint16_t* c1, const uint16_t* c2,
+                      const int32_t* b1, const int32_t* e1, const int32_t* b2, const int32_t* e2, const uint32_t* g1, const uint32_t* g2) {
+	ARB_API_BEGIN(ctx) ctx->e.set_blacklist(n, t1, t2, s1, s2, c1, c2, b1, e1, b2, e2, g1, g2); ARB_API_END(ctx)
+}
+int arb_filter_blacklist(arb_ctx* ctx, uint32_t n_ids, const uint32_t* ids, float evalue_cutoff, int32_t max_mate_gap, uint8_t* verdicts, uint32_t* n_blacklisted) {
+	ARB_API_BEGIN(ctx) const uint32_t b = ctx->e.filter_blacklist(n_ids, ids, evalue_cutoff, max_mate_gap, verdicts); if (n_blacklisted) *n_blacklisted = b; ARB_API_END(ctx)
+}
 int arb_get_slot_swaps(arb_ctx* ctx, uint8_t* out) { ARB_API_BEGIN(ctx) ctx->e.get_slot_swaps(out); ARB_API_END(ctx) }
 
 } // extern "C"

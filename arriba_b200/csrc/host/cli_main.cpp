@@ -1,6 +1,6 @@
 // cli_main.cpp -- the `arriba` command line of arriba-b200: same option letters, defaults and error texts as the reference
 // (options.cpp:270-485, usage options.cpp:109-268), driving the pipeline through the public C ABI only.
-// Not supported (fail loudly): -c Chimeric.out.sam, -b/-k/-t/-p database files, -G, -I.
+// Not supported (fail loudly): -c Chimeric.out.sam, -k/-t/-p database files, -G, -I.
 #include <getopt.h>
 #include <unistd.h>
 #include <sys/resource.h>
@@ -39,6 +39,7 @@ static void usage() {
 	          << " -x FILE  BAM with main and chimeric alignments (STAR --chimOutType WithinBAM)\n -g FILE  gene annotation (GTF)\n -a FILE  assembly (FastA)\n"
 	          << " -o FILE  output file   -O FILE  discarded candidates\n -f LIST  disable filters (comma/space separated)\n -s MODE  strandedness auto|yes|no|reverse\n"
 	          << " -i/-v contig lists, -E e-value cutoff, -S min support, -m/-L/-H/-R/-A/-M/-K/-V/-F/-U/-Q/-e/-l/-z/-Z thresholds as in the reference\n"
+	          << " -b FILE  blacklist (optionally .gz; required unless '-f blacklist')\n"
 	          << " -d FILE  genomic breakpoints from whole-genome sequencing (four-column or VCF, optionally .gz)\n -D N     maximum genomic breakpoint distance (default 100000)\n"
 	          << " -@ N     host threads for decoding and annotation   -u external duplicate marking   -X extra info for discarded candidates\n";
 }
@@ -63,7 +64,7 @@ int main(int argc, char** argv) {
 			case 'a': fasta = optarg; crash(access(optarg, R_OK), "file not found/readable: " + fasta); break;
 			case 'o': out = optarg; break;
 			case 'O': discarded = optarg; break;
-			case 'b': blacklist = optarg; break;
+			case 'b': blacklist = optarg; crash(access(optarg, R_OK), "file not found/readable: " + blacklist); break;
 			case 'd': genomic = optarg; crash(access(optarg, R_OK), "file not found/readable: " + genomic); break;
 			case 'D': crash(!int_in(optarg, 0, INT_MAX, iv), "invalid argument to " + opt); o.max_genomic_breakpoint_distance = (uint32_t) iv; break;
 			case 'c': case 't': case 'p': case 'k': case 'G': case 'I':
@@ -114,11 +115,11 @@ int main(int argc, char** argv) {
 	crash(fasta.empty(), "missing mandatory option -a");
 	const bool blacklist_on = o.params.filter_mask >> 20 & 1;
 	crash(blacklist_on && blacklist.empty(), "filter 'blacklist' enabled, but missing option -b (use '-f blacklist' if you want to disable the blacklist)");
-	crash(!blacklist.empty(), "option -b is not supported by arriba-b200: the blacklist database is not part of the reference repository (use '-f blacklist')");
 	o.bam_file = bam.c_str(); o.gtf_file = gtf.c_str(); o.assembly_file = fasta.c_str(); o.output_file = out.c_str();
 	o.discarded_output_file = discarded.empty() ? NULL : discarded.c_str();
 	o.interesting_contigs = interesting.empty() ? NULL : interesting.c_str(); o.viral_contigs = viral.empty() ? NULL : viral.c_str();
 	o.genomic_breakpoints_file = genomic.empty() ? NULL : genomic.c_str();
+	o.blacklist_file = blacklist.empty() ? NULL : blacklist.c_str();
 
 	arb_pipeline* p = NULL;
 	crash(arb_pipeline_create(&p, &o) != 0, arb_pipeline_error(NULL));

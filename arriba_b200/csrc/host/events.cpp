@@ -762,6 +762,25 @@ void pipeline::recover_genomic_support() { // filter_genomic_support.cpp:421-444
 	log_remaining("Searching for fusions with support from WGS");
 }
 
+// ------------------------------------------------------------------------------------------- blacklist (-b)
+// filter_blacklisted_ranges.cpp:232-300: the eligible set is fixed first, then the file is read (its warnings follow those of -d) and the rules are matched on the
+// device (csrc/blacklist_hd.h). The device reads the split-read / discordant-mate counts and e-values it holds: estimate_evalues (EV_EVALUE, always run) left the
+// host's there and no later stage changes them on the host; breakpoints, directions, genes and the spliced / strand bits never change after find_fusions.
+void pipeline::filter_blacklist() {
+	std::vector<u32> ids;
+	for (u32 k = 0; k < ev.n; ++k) if (ev.filter[k] == F_none || ev.genomic_support(k)) ids.push_back(k); // :238-239
+	fusion_rules r;
+	read_fusion_rules(opt.blacklist_file, ref, max_mate_gap, r);
+	const uint32_t n = (uint32_t) r.size();
+	check(ctx, arb_set_blacklist(ctx, n, r.type1.data(), r.type2.data(), r.strand1.data(), r.strand2.data(), r.contig1.data(), r.contig2.data(),
+	                             r.start1.data(), r.end1.data(), r.start2.data(), r.end2.data(), r.gene1.data(), r.gene2.data()), "arb_set_blacklist");
+	std::vector<u8> verdict(ids.size());
+	uint32_t blacklisted = 0;
+	check(ctx, arb_filter_blacklist(ctx, (uint32_t) ids.size(), ids.data(), opt.params.evalue_cutoff, max_mate_gap, verdict.data(), &blacklisted), "arb_filter_blacklist");
+	for (size_t x = 0; x < ids.size(); ++x) if (verdict[x]) ev.filter[ids[x]] = F_blacklist; // overwrites an earlier filter of a candidate with genomic support
+	log_remaining(("Filtering blacklisted fusions in '" + opt.blacklist_file + "'").c_str());
+}
+
 void pipeline::assign_confidence() { // filter_genomic_support.cpp:222-402
 	// the candidates of every gene (only counted below, so their order does not matter): one CSR table instead of a vector per gene
 	struct gene_list { const u32* p; size_t n; size_t size() const { return n; } u32 operator[](size_t x) const { return p[x]; } };

@@ -45,4 +45,13 @@ struct event_table {
 struct genomic_records { std::vector<u16> contig1, contig2; std::vector<u8> dir1, dir2; std::vector<i32> pos1, pos2; };
 void read_genomic_breakpoints(const std::string& path, const std::map<std::string, u16>& contigs, genomic_records& out);
 
+// rules of a blacklist file (blacklist.cpp), in file order: the two items of every line that parse_blacklist_item accepted, one column per field (type: ARB_RULE_*,
+// strand: ARB_RULE_STRAND_*, coordinates 0-based; gene: the gene of a GENE item). Lines it rejects print the reference's WARNING on stderr. A file of known
+// fusions (-k) has the same format.
+struct fusion_rules {
+	std::vector<u8> type1, type2, strand1, strand2; std::vector<u16> contig1, contig2; std::vector<i32> start1, end1, start2, end2; std::vector<u32> gene1, gene2;
+	size_t size() const { return type1.size(); }
+};
+void read_fusion_rules(const std::string& path, const refdata& ref, i32 max_mate_gap, fusion_rules& out);
+
 }} // namespace

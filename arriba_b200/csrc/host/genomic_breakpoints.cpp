@@ -1,33 +1,10 @@
 // genomic_breakpoints.cpp -- the file of genomic breakpoints from whole-genome sequencing (-d), read like mark_genomic_support does
 // (filter_genomic_support.cpp:80-167): Arriba's four-column format or a VCF (BND in bracket notation, DEL / DUP / INV with END), one record per line.
 // The records go to the device in file order (arb_set_genomic_breakpoints), which sorts them and searches them per candidate (csrc/genomic_hd.h).
-#include <climits>
-#include <cstdlib>
 #include <iostream>
 #include "events.h"
 
 namespace arb { namespace host {
-
-// tsv_stream_t (read_compressed_file.cpp:65-89): fields split at every tab, a missing field fails
-struct tsv_fields {
-	const std::string& s; size_t at; bool failed;
-	explicit tsv_fields(const std::string& line): s(line), at(0), failed(false) {}
-	std::string next() {
-		if (at >= s.size()) { failed = true; return std::string(); }
-		const size_t start = at; at = s.find('\t', start);
-		std::string out = s.substr(start, at - start);
-		if (at < s.size()) ++at;
-		return out;
-	}
-};
-
-// str_to_int (common.hpp:316-321): a long that fits is truncated to int
-static bool str_to_int(const std::string& text, i32& v) {
-	const char* s = text.c_str(); char* e;
-	const long r = strtol(s, &e, 10);
-	v = (i32) r;
-	return *s != ' ' && e != s && *e == '\0' && r != LONG_MAX && r != LONG_MIN;
-}
 
 // parse_breakpoint (:15-35): contig up to the LAST colon, without "chr", known to the run; position made 0-based
 static bool parse_breakpoint(std::string bp, const std::map<std::string, u16>& contigs, u16& contig, i32& position) {
@@ -68,13 +45,8 @@ void read_genomic_breakpoints(const std::string& path, const std::map<std::strin
 	auto add = [&](u16 c1, u16 c2, u8 d1, u8 d2, i32 p1, i32 p2) {
 		out.contig1.push_back(c1); out.contig2.push_back(c2); out.dir1.push_back(d1); out.dir2.push_back(d2); out.pos1.push_back(p1); out.pos2.push_back(p2);
 	};
-	size_t at = 0;
-	while (at < text.size()) {
-		size_t nl = text.find('\n', at);
-		if (nl == std::string::npos) nl = text.size();
-		std::string line = text.substr(at, nl - at);
-		at = nl + 1;
-		if (!line.empty() && line[line.size() - 1] == '\r') line.resize(line.size() - 1);
+	size_t at = 0; std::string line;
+	while (next_line(text, at, line)) {
 		if (line.empty() || line[0] == '#') continue;
 
 		u16 c1 = 0, c2 = 0; i32 p1 = 0, p2 = 0; u8 d1 = 0, d2 = 0;

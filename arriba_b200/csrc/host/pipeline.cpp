@@ -197,8 +197,9 @@ void pipeline::events_until(int last) { // arriba.cpp:420-545, filters enabled b
 			case EV_SELECT_BEST: if (on(F_select_best)) select_best(); break;
 			case EV_MARGINAL_READ_THROUGH: if (on(F_marginal_read_through)) filter_marginal_read_through(); break;
 			case EV_MANY_SPLICED: if (on(F_many_spliced)) recover_many_spliced(); break;
-			case EV_SHORT_ANCHOR: // arriba.cpp:516-523, then the short-anchor filter
+			case EV_SHORT_ANCHOR: // arriba.cpp:516-530, then the short-anchor filter
 				if (genomic && on(F_no_genomic_support)) { assign_confidence(); filter_no_genomic_support(); }
+				if (on(F_blacklist) && !opt.blacklist_file.empty()) filter_blacklist();
 				if (on(F_short_anchor)) filter_short_anchor();
 				break;
 			case EV_END_TO_END: if (on(F_end_to_end)) filter_end_to_end(); break;

@@ -35,6 +35,7 @@ struct run_options { // options_t (options.hpp:25-69) restricted to what this im
 	int min_support; unsigned min_anchor_length, min_spliced_events, min_itd_support; float high_expression_quantile, exonic_fraction, min_itd_allele_fraction; bool echo_progress;
 	unsigned top_viral_contigs; float viral_contig_min_covered_fraction; // -T 5, -C 0.05
 	std::string genomic_breakpoints_file; unsigned max_genomic_breakpoint_distance; // -d (empty: none), -D 100000
+	std::string blacklist_file; // -b (empty: none)
 	run_options();
 };
 
@@ -69,6 +70,7 @@ struct pipeline {
 	void filter_both_intronic(); void filter_in_vitro(); void recover_both_spliced(); void select_best(); void filter_marginal_read_through();
 	void recover_many_spliced(); void filter_short_anchor(); void filter_end_to_end(); void filter_no_coverage(); void recover_isoforms(); void assign_confidence();
 	void mark_genomic_support(); void filter_no_genomic_support(); void recover_genomic_support(); // -d (filter_genomic_support.cpp)
+	void filter_blacklist(); // -b (filter_blacklisted_ranges.cpp)
 	void write_output();
 	void make_kmer_index(); void filter_homologs(); void filter_mismappers(); bool splice_sites_ready;
 	void find_top_expressed_genes(std::vector<u32>& reads_by_gene, std::vector<u8>& present, unsigned int& threshold, float quantile);

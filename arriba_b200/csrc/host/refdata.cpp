@@ -10,10 +10,28 @@
 #include <stdexcept>
 #include <tuple>
 #include <climits>
+#include <cstdlib>
 
 namespace arb { namespace host {
 
 static void fail(const std::string& msg) { throw std::runtime_error(msg); }
+
+bool next_line(const std::string& text, size_t& at, std::string& line) {
+	if (at >= text.size()) return false;
+	size_t nl = text.find('\n', at);
+	if (nl == std::string::npos) nl = text.size();
+	line.assign(text, at, nl - at);
+	at = nl + 1;
+	if (!line.empty() && line[line.size() - 1] == '\r') line.resize(line.size() - 1);
+	return true;
+}
+
+bool str_to_int(const std::string& text, i32& v) {
+	const char* s = text.c_str(); char* e;
+	const long r = strtol(s, &e, 10);
+	v = (i32) r;
+	return *s != ' ' && e != s && *e == '\0' && r != LONG_MAX && r != LONG_MIN;
+}
 
 // ------------------------------------------------------------------------------------------- contig names and patterns
 std::string remove_chr(std::string contig) { // common.hpp:74-80

@@ -61,4 +61,23 @@ struct refdata {
 std::vector<std::string> read_lines_autodecompress(const std::string& path, std::string& storage);
 void read_whole_file(const std::string& path, std::string& out);
 
+// the line at `at` of a file read whole, without its '\n' and a trailing '\r' (autodecompress_file_t::getline, read_compressed_file.cpp:47-63); false at the end
+bool next_line(const std::string& text, size_t& at, std::string& line);
+
+// tsv_stream_t (read_compressed_file.cpp:65-89): fields split at every delimiter, a missing field fails
+struct tsv_fields {
+	const std::string& s; char delimiter; size_t at; bool failed;
+	explicit tsv_fields(const std::string& line, char d = '\t'): s(line), delimiter(d), at(0), failed(false) {}
+	std::string next() {
+		if (at >= s.size()) { failed = true; return std::string(); }
+		const size_t start = at; at = s.find(delimiter, start);
+		std::string out = s.substr(start, at - start);
+		if (at < s.size()) ++at;
+		return out;
+	}
+};
+
+// str_to_int (common.hpp:316-321): a long that fits is truncated to int
+bool str_to_int(const std::string& text, i32& v);
+
 }} // namespace

@@ -66,7 +66,7 @@ class Timings(C.Structure):
                 ("mismapper_items", C.c_uint64), ("kmer_positions", C.c_uint64), ("mismapper_heavy_items", C.c_uint64),
                 ("mismappers_pass1_ms", C.c_float), ("mismappers_pass2_ms", C.c_float), ("mismapper_tasks", C.c_uint64), ("mismapper_rounds", C.c_uint32), ("mismapper_overflow", C.c_uint32), ("mismapper_table_slots", C.c_uint32),
                 ("cascade_head_ms", C.c_float), ("cascade_sequences_ms", C.c_float), ("cascade_queued", C.c_uint64), ("cascade_algorithmic_bytes", C.c_uint64 * 2), ("annotate_ms", C.c_float), ("in_vitro_ms", C.c_float), ("multimappers_ms", C.c_float), ("order_ms", C.c_float), ("partners_ms", C.c_float), ("rows_ms", C.c_float), ("bam_scan_ms", C.c_float), ("consensus_ms", C.c_float), ("mismapper_algorithmic_bytes", C.c_uint64), ("mismapper_sequences", C.c_uint64), ("mismapper_hits", C.c_uint64),
-                ("genomic_support_ms", C.c_float)]
+                ("genomic_support_ms", C.c_float), ("blacklist_ms", C.c_float)]
 
 
 _CTYPE = {np.dtype(np.uint8): C.c_uint8, np.dtype(np.uint16): C.c_uint16, np.dtype(np.uint32): C.c_uint32, np.dtype(np.int32): C.c_int32,
@@ -129,6 +129,8 @@ def load(path=None):
                        ("arb_filter_mismappers_part", [C.c_int32, C.c_int, C.c_int, _p(C.c_void_p), _p(C.c_uint64)]), ("arb_filter_mismappers_finish", [_p(C.c_uint64)]),
                        ("arb_set_genomic_breakpoints", [C.c_uint32, _p(C.c_uint16), _p(C.c_uint16), _p(C.c_uint8), _p(C.c_uint8), _p(C.c_int32), _p(C.c_int32)]),
                        ("arb_mark_genomic_support", [C.c_int32, C.c_int32, _p(C.c_uint32)]), ("arb_get_genomic_support", [_p(C.c_int32), _p(C.c_int32)]),
+                       ("arb_set_blacklist", [C.c_uint32] + [_p(C.c_uint8)] * 4 + [_p(C.c_uint16)] * 2 + [_p(C.c_int32)] * 4 + [_p(C.c_uint32)] * 2),
+                       ("arb_filter_blacklist", [C.c_uint32, _p(C.c_uint32), C.c_float, C.c_int32, _p(C.c_uint8), _p(C.c_uint32)]),
                        ("arb_set_candidate_state", [_p(C.c_uint8), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_float)]),
                        ("arb_set_candidate_lists", [_p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32)]),
                        ("arb_set_splice_sites", [_p(C.c_uint32), _p(C.c_int32)]),
@@ -333,6 +335,25 @@ class Context:
         self._check(self.lib.arb_get_genomic_support(self.h, ptr(a), ptr(b)))
         return a[:n.value], b[:n.value]
 
+    # ---- blacklist (-b)
+    RULE_COLUMNS = (("type1", np.uint8), ("type2", np.uint8), ("strand1", np.uint8), ("strand2", np.uint8), ("contig1", np.uint16), ("contig2", np.uint16),
+                    ("start1", np.int32), ("end1", np.int32), ("start2", np.int32), ("end2", np.int32), ("gene1", np.uint32), ("gene2", np.uint32))
+
+    def set_blacklist(self, rules):
+        """rules: dict of the columns in RULE_COLUMNS, one entry per rule in file order (types and strands as ARB_RULE_* / ARB_RULE_STRAND_*, coordinates 0-based)."""
+        cols = [np.ascontiguousarray(rules[k], dt) for k, dt in self.RULE_COLUMNS]
+        n = cols[0].size
+        assert all(c.size == n for c in cols), "columns differ in length"
+        cols = [c if c.size else np.zeros(1, c.dtype) for c in cols]
+        self._check(self.lib.arb_set_blacklist(self.h, n, *[ptr(c) for c in cols]))
+
+    def filter_blacklist(self, ids, evalue_cutoff=3.0, max_mate_gap=0):
+        """Verdicts (1 = blacklisted) of the candidates `ids` against the rules of set_blacklist."""
+        ids = np.ascontiguousarray(ids, np.uint32)
+        out = np.zeros(max(ids.size, 1), np.uint8); n = C.c_uint32()
+        self._check(self.lib.arb_filter_blacklist(self.h, ids.size, ptr(ids if ids.size else np.zeros(1, np.uint32)), float(evalue_cutoff), int(max_mate_gap), ptr(out), C.byref(n)))
+        return out[:ids.size]
+
     def slot_swaps(self):
         s = np.zeros(self.n_fragments, np.uint8)
         self._check(self.lib.arb_get_slot_swaps(self.h, ptr(s)))
@@ -395,7 +416,7 @@ class RunOptions(C.Structure):
                 ("exonic_fraction", C.c_float), ("min_itd_allele_fraction", C.c_float), ("min_itd_support", C.c_uint32),
                 ("print_extra_info_for_discarded_fusions", C.c_int32), ("echo_progress", C.c_int32),
                 ("top_viral_contigs", C.c_uint32), ("viral_contig_min_covered_fraction", C.c_float),
-                ("genomic_breakpoints_file", C.c_char_p), ("max_genomic_breakpoint_distance", C.c_uint32)]
+                ("genomic_breakpoints_file", C.c_char_p), ("max_genomic_breakpoint_distance", C.c_uint32), ("blacklist_file", C.c_char_p)]
 
 
 class RunStats(C.Structure):
@@ -441,7 +462,7 @@ class Pipeline:
     """One run of the hot path on files: the call a user of the library makes (the `arriba` CLI is a thin wrapper over it)."""
 
     def __init__(self, bam, gtf, fasta, threads=1, device=0, lib_path=None, strandedness=3, params=None, output=None, discarded=None,
-                 genomic_breakpoints=None, max_genomic_breakpoint_distance=100000):
+                 genomic_breakpoints=None, max_genomic_breakpoint_distance=100000, blacklist=None):
         self.lib = load(lib_path)
         _load_pipeline_api(self.lib)
         o = RunOptions()
@@ -455,6 +476,8 @@ class Pipeline:
         if genomic_breakpoints:
             self._strings.append(genomic_breakpoints.encode()); o.genomic_breakpoints_file = self._strings[-1]
         o.max_genomic_breakpoint_distance = max_genomic_breakpoint_distance
+        if blacklist:  # read only while the blacklist filter is on (params.filter_mask bit 20)
+            self._strings.append(blacklist.encode()); o.blacklist_file = self._strings[-1]
         o.threads = threads; o.device = device; o.strandedness = strandedness
         if params is not None:
             o.params = params

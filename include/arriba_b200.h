@@ -307,6 +307,22 @@ int arb_set_genomic_breakpoints(arb_ctx* ctx, uint32_t n, const uint16_t* contig
 int arb_mark_genomic_support(arb_ctx* ctx, int32_t max_distance, int32_t max_itd_length, uint32_t* marked);
 int arb_get_genomic_support(arb_ctx* ctx, int32_t* closest1, int32_t* closest2);
 
+/* ---- blacklist (-b) -----------------------------------------------------------------------------------------------------------------------------------------
+ * arb_set_blacklist replaces the file loop of filter_blacklisted_ranges (source/filter_blacklisted_ranges.cpp:252-268): the rules that parse_blacklist_item
+ * (:83-120) accepted, in file order, as columns of their two items. type: ARB_RULE_*; strand: ARB_RULE_STRAND_* (positions and ranges only); contig, start
+ * and end (0-based, inclusive) of positions, ranges and genes; gene: the gene id of a GENE item. Fields an item type does not use are ignored.
+ * arb_filter_blacklist replaces the bins and the matching (:232-250, :270-292, matches_blacklist_item :138-223) over the resident candidate table: one verdict
+ * byte per id in `ids` (the caller's eligible candidates: no filter yet, or closest_genomic_breakpoint1 >= 0), 1 = blacklisted; *n_blacklisted counts them.
+ * The resident split-read / discordant-mate counts and e-values are the ones the candidate-state calls last left on the device. */
+enum { ARB_RULE_RANGE = 0, ARB_RULE_POSITION = 1, ARB_RULE_GENE = 2, ARB_RULE_ANY = 3, ARB_RULE_SPLIT_READ_DONOR = 4, ARB_RULE_SPLIT_READ_ACCEPTOR = 5,
+       ARB_RULE_SPLIT_READ_ANY = 6, ARB_RULE_DISCORDANT_MATES = 7, ARB_RULE_READ_THROUGH = 8, ARB_RULE_LOW_SUPPORT = 9, ARB_RULE_FILTER_SPLICED = 10,
+       ARB_RULE_NOT_BOTH_SPLICED = 11 };
+enum { ARB_RULE_STRAND_NONE = 0, ARB_RULE_STRAND_FORWARD = 1, ARB_RULE_STRAND_REVERSE = 2 };
+int arb_set_blacklist(arb_ctx* ctx, uint32_t n, const uint8_t* type1, const uint8_t* type2, const uint8_t* strand1, const uint8_t* strand2,
+                      const uint16_t* contig1, const uint16_t* contig2, const int32_t* start1, const int32_t* end1, const int32_t* start2, const int32_t* end2,
+                      const uint32_t* gene1, const uint32_t* gene2);
+int arb_filter_blacklist(arb_ctx* ctx, uint32_t n_ids, const uint32_t* ids, float evalue_cutoff, int32_t max_mate_gap, uint8_t* verdicts, uint32_t* n_blacklisted);
+
 /* ---- device timing (CUDA events recorded on the context's stream around each stage) ---------------------------------- */
 typedef struct arb_timings {
 	float duplicates_ms;        /* duplicate marking (key build + hash group-by + mark) */
@@ -336,6 +352,7 @@ typedef struct arb_timings {
 	uint64_t mismapper_algorithmic_bytes; /* SURVEY.md section 8(d) budget of pass 1 of the re-alignment: per searched sequence of length l, 3l/8 + 8(l-8) + 4*hits + l/2 */
 	uint64_t mismapper_sequences, mismapper_hits; /* sequences searched by pass 1 (segment x gene x strand) and k-mer hits they visited */
 	float genomic_support_ms;   /* arb_mark_genomic_support: search of the sorted genomic breakpoints and the copy of the marks */
+	float blacklist_ms;         /* arb_filter_blacklist: key table of the rules, the search and the copy of the verdicts */
 } arb_timings;
 int arb_get_timings(arb_ctx* ctx, arb_timings* out);
 /* Device scratch memory is pooled per device and survives arb_ctx_destroy so that the next sample reuses it; this returns it to the driver
@@ -376,6 +393,7 @@ typedef struct arb_run_options {
 	float viral_contig_min_covered_fraction; /* -C 0.05 */
 	const char* genomic_breakpoints_file;    /* -d: structural variants from whole-genome sequencing (four-column or VCF, optionally .gz), NULL = none */
 	uint32_t max_genomic_breakpoint_distance; /* -D 100000 */
+	const char* blacklist_file;      /* -b: blacklist rules (optionally .gz), NULL = none; read only while the blacklist filter is on */
 } arb_run_options;
 void arb_default_run_options(arb_run_options* o);
 
