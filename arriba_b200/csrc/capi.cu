@@ -1,6 +1,9 @@
 // capi.cu -- the C ABI declared in include/arriba_b200.h: thin exception-to-status shims over arb::engine.
 #include "engine.h"
 #include <new>
+#include <map>
+#include <mutex>
+#include <sys/mman.h>
 
 using namespace arb;
 
@@ -13,13 +16,30 @@ static std::string g_create_error;
 namespace arb { namespace host { void set_host_block_backend(void* (*alloc)(size_t), void (*release)(void*)); } }
 static int g_host_memory_device = -1;
 #ifdef ARB_DEVICE_BUILD
+// The blocks are mapped by the process, asked for 2 MiB pages (THP "madvise") and then registered with the driver: the ingest's record loop visits its
+// workers' pools (hundreds of megabytes, page-locked so that they go to the device at full speed) all over, and on 4 KiB pages nearly every visit would
+// also miss the TLB. Where the kernel grants no huge pages the block is page-locked all the same.
+namespace { struct pinned_blocks { std::mutex lock; std::map<void*, std::pair<void*, size_t> > mapping; }; pinned_blocks& pinned() { static pinned_blocks* b = new pinned_blocks(); return *b; } }
 static void* pinned_alloc(size_t bytes) {
 	if (g_host_memory_device >= 0) { int cur = -1; if (cudaGetDevice(&cur) != cudaSuccess || cur != g_host_memory_device) { if (cudaSetDevice(g_host_memory_device) != cudaSuccess) { cudaGetLastError(); return NULL; } } }
-	void* p = NULL;
-	if (cudaHostAlloc(&p, bytes, cudaHostAllocPortable) != cudaSuccess) { cudaGetLastError(); return NULL; }
+	const size_t huge = (size_t) 2 << 20, len = ((bytes ? bytes : 1) + huge - 1) & ~(huge - 1);
+	void* base = mmap(NULL, len + huge, PROT_READ | PROT_WRITE, MAP_PRIVATE | MAP_ANONYMOUS, -1, 0);
+	if (base == MAP_FAILED) return NULL;
+	void* p = (void*) (((uintptr_t) base + huge - 1) & ~(uintptr_t) (huge - 1));
+#ifdef MADV_HUGEPAGE
+	madvise(p, len, MADV_HUGEPAGE);
+#endif
+	if (cudaHostRegister(p, len, cudaHostRegisterPortable) != cudaSuccess) { cudaGetLastError(); munmap(base, len + huge); return NULL; }
+	std::lock_guard<std::mutex> g(pinned().lock);
+	pinned().mapping[p] = std::make_pair(base, len + huge);
 	return p;
 }
-static void pinned_free(void* p) { cudaFreeHost(p); }
+static void pinned_free(void* p) {
+	std::pair<void*, size_t> m(NULL, 0);
+	{ std::lock_guard<std::mutex> g(pinned().lock); std::map<void*, std::pair<void*, size_t> >::iterator it = pinned().mapping.find(p); if (it == pinned().mapping.end()) return; m = it->second; pinned().mapping.erase(it); }
+	cudaHostUnregister(p);
+	munmap(m.first, m.second);
+}
 namespace { struct install_pinned_backend { install_pinned_backend() { arb::host::set_host_block_backend(pinned_alloc, pinned_free); } } g_install_pinned_backend; }
 #endif
 
@@ -84,6 +104,9 @@ int arb_set_contig_flags(arb_ctx* ctx, const uint8_t* flags, uint32_t n) { ARB_A
 int arb_push_chunk(arb_ctx* ctx, const arb_soa_chunk* c) { ARB_API_BEGIN(ctx) ctx->e.push_chunk(*c); ARB_API_END(ctx) }
 int arb_push_chunk_begin(arb_ctx* ctx, const arb_soa_chunk* c) { ARB_API_BEGIN(ctx) ctx->e.push_chunk_begin(*c); ARB_API_END(ctx) }
 int arb_push_chunk_end(arb_ctx* ctx, const arb_soa_chunk* c) { ARB_API_BEGIN(ctx) ctx->e.push_chunk_end(*c); ARB_API_END(ctx) }
+int arb_fragment_pools_upload(arb_ctx* ctx, const arb_fragment_pools* pools, uint32_t n_pools) { ARB_API_BEGIN(ctx) ctx->e.fragment_pools_upload(pools, n_pools); ARB_API_END(ctx) }
+int arb_fragment_table_build(arb_ctx* ctx, uint64_t sizes[6]) { ARB_API_BEGIN(ctx) ctx->e.fragment_table_build(sizes); ARB_API_END(ctx) }
+int arb_fragment_table_download(arb_ctx* ctx, const arb_soa_chunk* columns, char* names, uint64_t* name_off) { ARB_API_BEGIN(ctx) ctx->e.fragment_table_download(*columns, names, name_off); ARB_API_END(ctx) }
 int arb_bam_scan(arb_ctx* ctx, const uint8_t* chunk, uint64_t bytes, uint64_t first, int32_t n_ref, uint32_t n_lists, uint64_t* consumed, uint32_t* n_records, uint32_t* list_begin, uint32_t* record_offsets, uint32_t* malformed) {
 	ARB_API_BEGIN(ctx) u64 c = 0; ctx->e.bam_scan(chunk, bytes, first, n_ref, n_lists, &c, n_records, list_begin, record_offsets, malformed); *consumed = c; ARB_API_END(ctx)
 }

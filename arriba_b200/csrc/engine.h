@@ -113,6 +113,12 @@ public:
 	void get_annotation_columns(u8* aflags, u32* genes_off, u16* genes_cnt, u32* genes);
 	dbuf<u32> annot_rows, annot_pool, annot_ctl; dbuf<u16> annot_cnt; u32 annot_pool_cap, n_dummy; u64 n_gene_entries; dbuf<u16> dummy_contig; dbuf<i32> dummy_start, dummy_end;
 	void finish_push(u64 n_gene_ids); u64 push_cigar_ops; dbuf<u64> chunk_stats;
+	void adopt_table(const exec_ctx& cx, u64 n_cigar, u64 n_seq_bytes); // the columns in `frags` become the resident table (statistics, push_open)
+	// the fragment table built from the ingest workers' pools (fragtable.cu)
+	void fragment_pools_upload(const arb_fragment_pools* pools, u32 n_pools); void fragment_table_build(u64 sizes[6]);
+	void fragment_table_download(const arb_soa_chunk& columns, char* names, u64* name_off);
+	dbuf<arb_pool_fragment> pool_frags; dbuf<arb_pool_alignment> pool_alns; dbuf<char> pool_names, frag_names; dbuf<u32> pool_cigars; dbuf<u8> pool_seqs;
+	dbuf<u64> pool_base, frag_name_off; u32 pool_workers; u64 frag_name_bytes;
 	// one sample on several GPUs (exchange.cu): replicated state travels as groups of device buffers, the work of find_fusions / filter_mismappers is divided
 	void exchange_header(int group, std::vector<u64>& header); void exchange_prepare(int group, const u64* header, u32 n_words);
 	void exchange_buffers(int group, std::vector<exchange_buffer>& out); void exchange_commit(int group);

@@ -31,7 +31,7 @@ void* host_block_get(size_t bytes, size_t& granted);
 void release_worker_cache(); // the ingest keeps the workers' pools of a finished sample for the next one (ingest.cpp)
 void host_block_put(void* p, size_t granted);
 void host_block_trim();
-// where fresh blocks come from (default: malloc). The CUDA library installs cudaHostAlloc / cudaFreeHost (capi.cu); a NULL result falls back to malloc.
+// where fresh blocks come from (default: malloc). The CUDA library installs page-locked blocks on 2 MiB pages (capi.cu); a NULL result falls back to malloc.
 void set_host_block_backend(void* (*alloc)(size_t), void (*release)(void*));
 
 // vector whose resize() leaves new elements uninitialised: the large columns are first touched (and zeroed where needed) by the threads that fill them
@@ -71,7 +71,7 @@ struct fragment_table { // host image of arb_soa_chunk + names
 };
 
 struct ingest_stats {
-	u64 mapped_reads; std::vector<u64> mapped_viral_reads_by_contig; u64 malformed, missing_hi_tag, records; bool no_chimeric_reads;
+	u64 mapped_reads; std::vector<u64> mapped_viral_reads_by_contig; u64 malformed, missing_hi_tag, records, multimapper_pairs /* neighbours with the same read name */; bool no_chimeric_reads;
 	double t_inflate, t_parse, t_finalize;
 };
 

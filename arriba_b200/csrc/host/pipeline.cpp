@@ -60,16 +60,7 @@ void pipeline::annotate() {
 	const double t0 = now_s();
 	ref.set_contig_flags(opt.interesting_contigs, opt.viral_contigs);
 	ref.flatten();
-	u32 marked = 0;
-	for (u32 i = 0; i + 1 < frags.n; ++i) { // count adjacent pairs like mark_multimappers' return value
-		const u64 a0 = frags.name_off[i], a1 = frags.name_off[i + 1], a2 = frags.name_off[i + 2];
-		u64 la = a1 - a0, lb = a2 - a1;
-		while (la > 0 && frags.names[a0 + la - 1] != ',') --la;
-		while (lb > 0 && frags.names[a1 + lb - 1] != ',') --lb;
-		const u64 sa = la > 0 ? la - 1 : a1 - a0, sb = lb > 0 ? lb - 1 : a2 - a1;
-		if (sa == sb && std::equal(frags.names.begin() + a0, frags.names.begin() + a0 + sa, frags.names.begin() + a1)) ++marked;
-	}
-	{ std::ostringstream s; s << "Marking multi-mapping alignments (marked=" << marked << ")"; say(s.str()); }
+	{ std::ostringstream s; s << "Marking multi-mapping alignments (marked=" << istats.multimapper_pairs << ")"; say(s.str()); } // adjacent pairs, mark_multimappers' return value: counted where the flags are set (ingest)
 	strandedness = opt.strandedness;
 	if (opt.strandedness == 3) {
 		strandedness = detect_strandedness(*this);
@@ -96,23 +87,11 @@ void pipeline::upload_reference() {
 	reference_on_device = true; contigs_on_device = nc;
 }
 
-arb_soa_chunk pipeline::chunk_of(fragment_table& frags) {
-	arb_soa_chunk c;
-	c.n_fragments = frags.n; c.n_aln = frags.n_aln.data(); c.fflags = frags.fflags.data(); c.filter = frags.filter.data();
-	c.contig = frags.contig.data(); c.start = frags.start.data(); c.end = frags.end.data(); c.aflags = frags.aflags.data();
-	c.cigar_off = frags.cigar_off.data(); c.cigar_cnt = frags.cigar_cnt.data(); c.seq_off = frags.seq_off.data(); c.seq_len = frags.seq_len.data();
-	c.genes_off = frags.genes_off.data(); c.genes_cnt = frags.genes_cnt.data();
-	c.cigar = frags.cigar.data(); c.n_cigar = frags.cigar.size(); c.seq = frags.seq.data(); c.n_seq_bytes = frags.seq.size(); c.genes = frags.genes.data(); c.n_genes = frags.genes.size();
-	return c;
-}
-
-// end of ingest: the genome and every column ingest produced start their way to the device while the host annotates (the gene sets follow in upload())
+// end of ingest: the fragment table is already resident (ingest built it on the device); the contig table, complete once the BAM header has been read, follows
 void pipeline::begin_upload() {
-	ref.set_contig_flags(opt.interesting_contigs, opt.viral_contigs); // the contig table is complete once the BAM header has been read
+	ref.set_contig_flags(opt.interesting_contigs, opt.viral_contigs);
 	ref.flatten();
 	upload_reference();
-	arb_soa_chunk c = chunk_of(frags);
-	check(ctx, arb_push_chunk_begin(ctx, &c), "arb_push_chunk_begin");
 }
 
 // gene / exon tables and their region indices (after annotate(): with the dummy genes)

@@ -59,7 +59,7 @@ struct pipeline {
 	void ingest();
 	void annotate();
 	void upload();
-	void upload_reference(); void send_annotation(); void begin_upload(); arb_soa_chunk chunk_of(fragment_table& t); // ingest ends by starting the copy of its columns; annotation overlaps it
+	void upload_reference(); void send_annotation(); void begin_upload();
 	void read_filters();
 	void fragment_length();
 	void find_fusions();

@@ -144,6 +144,16 @@ public:
 		memcpy(p_, host, n * sizeof(T));
 #endif
 	}
+	void upload_at(const exec_ctx& ex, const T* host, size_t n, size_t offset) { // into [offset, offset + n) of a buffer already large enough
+		(void) ex;
+		if (!n) return;
+		if (offset + n > n_) throw arb_error("dbuf::upload_at past the end of the buffer");
+#ifdef ARB_DEVICE_BUILD
+		ARB_CUDA_CHECK(cudaMemcpyAsync(p_ + offset, host, n * sizeof(T), cudaMemcpyHostToDevice, ex.stream));
+#else
+		memcpy(p_ + offset, host, n * sizeof(T));
+#endif
+	}
 	void download(const exec_ctx& ex, T* host, size_t n, size_t offset = 0) const {
 		(void) ex;
 		if (!n) return;

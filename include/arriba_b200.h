@@ -105,7 +105,7 @@ int arb_push_chunk(arb_ctx* ctx, const arb_soa_chunk* chunk); /* H2D copy; repla
 /* The same in two parts, so that the copy overlaps the caller's annotation pass: _begin copies everything read_chimeric_alignments produced (all columns but
  * aflags and the gene sets) asynchronously on the context's copy stream; _end copies aflags / genes_off / genes_cnt / genes and returns when the table is
  * resident. The columns must stay valid and unchanged (apart from the annotation columns) between the two calls. Copies are asynchronous when the columns
- * are page-locked; the whole-run driver builds them in page-locked blocks (cudaHostAlloc, recycled across samples). */
+ * are page-locked; the whole-run driver builds them in page-locked blocks (registered with cudaHostRegister, recycled across samples). */
 int arb_push_chunk_begin(arb_ctx* ctx, const arb_soa_chunk* chunk);
 int arb_push_chunk_end(arb_ctx* ctx, const arb_soa_chunk* chunk);
 /* ---- BAM records of an inflated chunk -------------------------------------------------------------------------
@@ -116,6 +116,28 @@ int arb_push_chunk_end(arb_ctx* ctx, const arb_soa_chunk* chunk);
  * record_offsets: capacity bytes / 36 + 1; malformed != 0: a block_size < 33 was met where a one-thread walk would have met it. */
 int arb_bam_scan(arb_ctx* ctx, const uint8_t* chunk, uint64_t bytes, uint64_t first, int32_t n_ref, uint32_t n_lists, uint64_t* consumed, uint32_t* n_records,
                  uint32_t* list_begin /* n_lists + 1 */, uint32_t* record_offsets, uint32_t* malformed);
+/* ---- fragment table from the pools of the ingest's workers ---------------------------------------------------------
+ * What the record loop of ingest leaves per worker: fragments (name, chain of alignments in arrival order) and pools of names, CIGAR operations and nt16
+ * sequences. Offsets and links are local to the worker. The device turns the pools of all workers into the resident fragment table: slot normalisation and
+ * rejection of malformed fragments (source/read_chimeric_alignments.cpp:340-506), name order (std::string::compare of "<qname>,<HI>[ITD]"), the SoA columns
+ * in the layout arb_push_chunk takes (sequences back to back in fragment order, slot 0 then slot 1) and the multimapper flags (:792-802).
+ *   arb_fragment_pools_upload : copies the pools (page-locked memory: at full PCIe speed) and returns when they are resident,
+ *   arb_fragment_table_build  : builds the table, which becomes the resident one (as after arb_push_chunk_begin); sizes = {fragments, rejected fragments,
+ *                               CIGAR operations, sequence bytes, name bytes, neighbours in name order with the same read name (mark_multimappers' count)},
+ *   arb_fragment_table_download : the host copy (caller-allocated: n, n, n, 3n; 3n, 3n, 3n, 3n, 3n; 2n, 2n; 3n, 3n; CIGAR operations + 1, sequence bytes;
+ *                               name bytes, n + 1 offsets). */
+typedef struct { uint8_t supplementary, first_in_pair, forward; uint16_t contig; int32_t start, end; uint32_t cigar_off, cigar_cnt; uint64_t seq_off; uint32_t seq_len; int32_t next; } arb_pool_alignment;
+typedef struct { uint64_t name_off; uint32_t name_len; int32_t head, tail; uint32_t count; uint8_t single_end, duplicate; } arb_pool_fragment;
+typedef struct {
+	const arb_pool_fragment* frags; uint64_t n_frags;
+	const arb_pool_alignment* alns; uint64_t n_alns;   /* `next` links a fragment's alignments, -1 ends the chain */
+	const char* names; uint64_t n_name_bytes;
+	const uint32_t* cigars; uint64_t n_cigars;
+	const uint8_t* seqs; uint64_t n_seq_bytes;         /* each sequence 16-byte aligned */
+} arb_fragment_pools;
+int arb_fragment_pools_upload(arb_ctx* ctx, const arb_fragment_pools* pools, uint32_t n_pools);
+int arb_fragment_table_build(arb_ctx* ctx, uint64_t sizes[6]);
+int arb_fragment_table_download(arb_ctx* ctx, const arb_soa_chunk* columns, char* names, uint64_t* name_off);
 /* ---- annotation of the resident fragments -------------------------------------------------------------------
  * Replaces the annotation passes of main (source/arriba.cpp:165-325: annotate_alignments per fragment, source/annotation.cpp:431-555; dummy genes for
  * intergenic breakpoints, arriba.cpp:207-260; second pass :262-319) and assign_strands_from_strandedness (source/read_chimeric_alignments.cpp:775-790).
