@@ -1,16 +1,13 @@
-// bamscan.cu -- BAM record boundaries of a chunk of inflated BGZF payload, read-name hashes and the per-worker record lists, on the device.
+// bamscan.cu -- BAM record boundaries of a chunk of inflated BGZF payload, on the device.
 //
 // A BAM record can only be found from the one before it (SAMv1 4.2: block_size, then the record). The reference reads record after record
-// (read_chimeric_alignments.cpp:611, sam_read1); the host-side ingest used to walk the chain on all threads and hash every read name in a second pass --
-// a quarter of the ingest's CPU time for pure bookkeeping. Here the chunk (already in page-locked memory) is copied to the device and
+// (read_chimeric_alignments.cpp:611, sam_read1). Here, on the chunk in device memory (records.cu copies it up),
 //   1. every 64 KB piece GUESSES its first record: the first offset from which three records in a row look sane (necessary conditions only);
 //   2. every piece hops from its guess to the next piece's guess, counting records;
 //   3. one thread VERIFIES: the chain of piece s must arrive exactly at the guess of piece s + 1; where it does not, that stretch is walked serially
 //      (errors are therefore raised exactly where a one-thread walk would raise them);
-//   4. every piece hops again from its verified start, writes the record offsets and hashes the read names (FNV-1a, the worker of a record is a
-//      function of its name, so mates meet in one worker);
-//   5. a stable 8-bit radix sort by worker turns the offsets into one list per worker, file order kept.
-// The host workers then parse their lists (csrc/host/ingest.cpp); what a record means stays there.
+//   4. every piece hops again from its verified start and writes the record offsets, in file order.
+// What a record means is records_hd.h / records.cu.
 #include <cstdlib>
 #include "engine.h"
 
@@ -74,36 +71,24 @@ struct bam_stitch_fn { // one thread: follows the true chain over the pieces
 		result[0] = cur; result[1] = total; result[2] = malformed ? 1 : 0;
 	}
 };
-struct bam_write_fn { // piece s: its records' offsets and workers
-	bam_chunk c; const u64* start; const u32* base; const u32* count; u32 n_shards; u32* rec_off; u32* rec_shard;
+struct bam_write_fn { // piece s: its records' offsets, file order
+	bam_chunk c; const u64* start; const u32* base; const u32* count; u32* rec_off;
 	ARB_HD void operator()(u32 s) const {
 		u64 q = start[s]; u32 at = base[s];
-		for (u32 k = 0; k < count[s]; ++k, ++at) {
-			const u32 bs = bam_rd32(c.B + q);
-			const u8* name = c.B + q + 36; const u32 lq = c.B[q + 12];
-			u64 h = 1469598103934665603ULL;
-			for (u32 x = 0; x + 1 < lq && name[x]; ++x) { h ^= name[x]; h *= 1099511628211ULL; }
-			rec_off[at] = (u32) q; rec_shard[at] = (u32) ((h >> 20) % (u64) n_shards);
-			q += 4 + (u64) bs;
-		}
+		for (u32 k = 0; k < count[s]; ++k, ++at) { rec_off[at] = (u32) q; q += 4 + (u64) bam_rd32(c.B + q); }
 	}
 };
-struct bam_shard_count_fn { const u32* shard; u32* count; ARB_HD void operator()(u32 k) const { atomic_add_u32(&count[shard[k]], 1); } };
 
-void engine::bam_scan(const u8* chunk, u64 bytes, u64 first, i32 n_ref, u32 n_shards, u64* consumed, u32* n_records, u32* shard_begin, u32* record_offsets, u32* malformed) {
-	if (bytes >= 0xFFFFFFF0ull) throw arb_error("arb_bam_scan: chunk too large");
-	if (n_shards == 0 || n_shards > 256) throw arb_error("arb_bam_scan: 1 to 256 lists");
+// the records of bytes [first, bytes) of `B` (device memory): rec_off gets their offsets in file order
+void engine::bam_scan(const u8* B, u64 bytes, u64 first, i32 n_ref, dbuf<u32>& rec_off, u64* consumed, u32* n_records, u32* malformed) {
+	if (bytes >= 0xFFFFFFF0ull) throw arb_error("failed to load alignments (chunk too large)");
 	*consumed = first; *n_records = 0; *malformed = 0;
-	for (u32 k = 0; k <= n_shards; ++k) shard_begin[k] = 0;
 	if (first >= bytes) return;
-	stage_timer t_all(ex);
-	bam_buf.ensure(bytes + 64);
-	bam_buf.upload(ex, chunk, bytes);
 	const u64 PIECE = getenv("ARB_BAM_SCAN_PIECE") ? (u64) std::max(1L, atol(getenv("ARB_BAM_SCAN_PIECE"))) : (u64) 64 << 10; // env: test hook (pieces smaller than a record)
 	const u64 span = bytes - first;
 	const u32 pieces = (u32) std::max<u64>(1, std::min<u64>(span / PIECE, 1u << 16));
 	const u64 piece_bytes = span / pieces;
-	bam_chunk c = {bam_buf.ptr(), bytes, n_ref};
+	bam_chunk c = {B, bytes, n_ref};
 	dbuf<u64> guess((size_t) pieces + 1), stop_at(pieces), start((size_t) pieces + 1), result(3);
 	dbuf<u32> count(pieces), base((size_t) pieces + 1); dbuf<u8> bad(pieces);
 	bam_guess_fn gf = {c, first, piece_bytes, pieces, guess.ptr()};
@@ -116,19 +101,10 @@ void engine::bam_scan(const u8* chunk, u64 bytes, u64 first, i32 n_ref, u32 n_sh
 	*consumed = res[0]; *malformed = (u32) res[2];
 	const u32 R = (u32) res[1];
 	*n_records = R;
-	if (res[2] || R == 0) { timings.bam_scan_ms += t_all.stop(); return; }
-	dbuf<u32> rec_off(R), rec_shard(R), tk(R), tv(R), shard_count((size_t) n_shards + 1);
-	bam_write_fn wf = {c, start.ptr(), base.ptr(), count.ptr(), n_shards, rec_off.ptr(), rec_shard.ptr()};
+	if (res[2] || R == 0) return;
+	rec_off.ensure(R);
+	bam_write_fn wf = {c, start.ptr(), base.ptr(), count.ptr(), rec_off.ptr()};
 	for_each(ex, pieces, wf);
-	shard_count.zero(ex, (size_t) n_shards + 1);
-	bam_shard_count_fn cf = {rec_shard.ptr(), shard_count.ptr()};
-	for_each(ex, R, cf);
-	radix_sort_pairs_u32(ex, rec_shard.ptr(), rec_off.ptr(), tk.ptr(), tv.ptr(), R, 8); // stable: file order inside a list
-	std::vector<u32> counts(n_shards);
-	shard_count.download(ex, counts.data(), n_shards);
-	for (u32 k = 0; k < n_shards; ++k) shard_begin[k + 1] = shard_begin[k] + counts[k];
-	rec_off.download(ex, record_offsets, R);
-	timings.bam_scan_ms += t_all.stop();
 }
 
 } // namespace arb

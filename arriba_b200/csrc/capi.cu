@@ -104,11 +104,20 @@ int arb_set_contig_flags(arb_ctx* ctx, const uint8_t* flags, uint32_t n) { ARB_A
 int arb_push_chunk(arb_ctx* ctx, const arb_soa_chunk* c) { ARB_API_BEGIN(ctx) ctx->e.push_chunk(*c); ARB_API_END(ctx) }
 int arb_push_chunk_begin(arb_ctx* ctx, const arb_soa_chunk* c) { ARB_API_BEGIN(ctx) ctx->e.push_chunk_begin(*c); ARB_API_END(ctx) }
 int arb_push_chunk_end(arb_ctx* ctx, const arb_soa_chunk* c) { ARB_API_BEGIN(ctx) ctx->e.push_chunk_end(*c); ARB_API_END(ctx) }
-int arb_fragment_pools_upload(arb_ctx* ctx, const arb_fragment_pools* pools, uint32_t n_pools) { ARB_API_BEGIN(ctx) ctx->e.fragment_pools_upload(pools, n_pools); ARB_API_END(ctx) }
 int arb_fragment_table_build(arb_ctx* ctx, uint64_t sizes[6]) { ARB_API_BEGIN(ctx) ctx->e.fragment_table_build(sizes); ARB_API_END(ctx) }
 int arb_fragment_table_download(arb_ctx* ctx, const arb_soa_chunk* columns, char* names, uint64_t* name_off) { ARB_API_BEGIN(ctx) ctx->e.fragment_table_download(*columns, names, name_off); ARB_API_END(ctx) }
-int arb_bam_scan(arb_ctx* ctx, const uint8_t* chunk, uint64_t bytes, uint64_t first, int32_t n_ref, uint32_t n_lists, uint64_t* consumed, uint32_t* n_records, uint32_t* list_begin, uint32_t* record_offsets, uint32_t* malformed) {
-	ARB_API_BEGIN(ctx) u64 c = 0; ctx->e.bam_scan(chunk, bytes, first, n_ref, n_lists, &c, n_records, list_begin, record_offsets, malformed); *consumed = c; ARB_API_END(ctx)
+int arb_records_begin(arb_ctx* ctx, const uint16_t* tid_to_contig, uint32_t n_tid, const uint8_t* interesting, const uint8_t* viral, const uint64_t* n_windows, uint32_t n_contigs,
+                      uint32_t max_itd_length, int external_duplicate_marking, uint64_t expected_bytes) {
+	ARB_API_BEGIN(ctx) std::vector<u64> w(n_windows, n_windows + n_contigs); ctx->e.records_begin(tid_to_contig, n_tid, interesting, viral, w.data(), n_contigs, max_itd_length, external_duplicate_marking != 0, expected_bytes); ARB_API_END(ctx)
+}
+int arb_records_chunk(arb_ctx* ctx, const uint8_t* chunk, uint64_t bytes, uint64_t first, uint64_t chunk_pos, uint64_t* n_records, uint64_t* carry, uint32_t* malformed, uint64_t* error) {
+	ARB_API_BEGIN(ctx) u64 r = 0, c = 0, e = 0; ctx->e.records_chunk(chunk, bytes, first, chunk_pos, &r, &c, malformed, &e); *n_records = r; *carry = c; *error = e; ARB_API_END(ctx)
+}
+int arb_records_error_record(arb_ctx* ctx, const uint8_t** body, uint64_t* bytes) {
+	ARB_API_BEGIN(ctx) *body = ctx->e.rec_error_record.data(); *bytes = ctx->e.rec_error_record.size(); ARB_API_END(ctx)
+}
+int arb_records_finish(arb_ctx* ctx, uint16_t* const* coverage, uint8_t* const* starts, uint8_t* const* ends, uint64_t* counters, uint64_t* error) {
+	ARB_API_BEGIN(ctx) u64 e = 0; ctx->e.records_finish(coverage, starts, ends, (u64*) counters, &e); *error = e; ARB_API_END(ctx)
 }
 int arb_annotate_pass1(arb_ctx* ctx, const uint8_t* aflags, int32_t strandedness, uint32_t* n_dummy) { ARB_API_BEGIN(ctx) const uint32_t k = ctx->e.annotate_pass1(aflags, strandedness); if (n_dummy) *n_dummy = k; ARB_API_END(ctx) }
 int arb_get_dummy_genes(arb_ctx* ctx, uint16_t* contig, int32_t* start, int32_t* end) { ARB_API_BEGIN(ctx) ctx->e.get_dummy_genes(contig, start, end); ARB_API_END(ctx) }

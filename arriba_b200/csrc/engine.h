@@ -114,8 +114,8 @@ public:
 	dbuf<u32> annot_rows, annot_pool, annot_ctl; dbuf<u16> annot_cnt; u32 annot_pool_cap, n_dummy; u64 n_gene_entries; dbuf<u16> dummy_contig; dbuf<i32> dummy_start, dummy_end;
 	void finish_push(u64 n_gene_ids); u64 push_cigar_ops; dbuf<u64> chunk_stats;
 	void adopt_table(const exec_ctx& cx, u64 n_cigar, u64 n_seq_bytes); // the columns in `frags` become the resident table (statistics, push_open)
-	// the fragment table built from the ingest workers' pools (fragtable.cu)
-	void fragment_pools_upload(const arb_fragment_pools* pools, u32 n_pools); void fragment_table_build(u64 sizes[6]);
+	// the fragment table built from the fragment pools the record replay wrote (fragtable.cu)
+	void fragment_table_build(u64 sizes[6]);
 	void fragment_table_download(const arb_soa_chunk& columns, char* names, u64* name_off);
 	dbuf<arb_pool_fragment> pool_frags; dbuf<arb_pool_alignment> pool_alns; dbuf<char> pool_names, frag_names; dbuf<u32> pool_cigars; dbuf<u8> pool_seqs;
 	dbuf<u64> pool_base, frag_name_off; u32 pool_workers; u64 frag_name_bytes;
@@ -144,8 +144,16 @@ public:
 	void filter_relative_support(float cutoff); void filter_multimappers(); u32 filter_simple(int stage, float exonic_fraction, int min_support); void evalue_tallies(u32* out); u32 select_best();
 	void replay_insertion_order(const u32* phase_start, const u64* phase_buckets, u32 n_phases, u32* order_out, u32* rank_out); dbuf<u32> order_rank;
 	void partner_counts(i32* count_out); dbuf<u32> order_seq;
-	// BAM record boundaries and per-worker record lists of an inflated chunk (bamscan.cu)
-	void bam_scan(const u8* chunk, u64 bytes, u64 first, i32 n_ref, u32 n_shards, u64* consumed, u32* n_records, u32* shard_begin, u32* record_offsets, u32* malformed); dbuf<u8> bam_buf;
+	// BAM record boundaries of an inflated chunk in device memory (bamscan.cu)
+	void bam_scan(const u8* B, u64 bytes, u64 first, i32 n_ref, dbuf<u32>& rec_off, u64* consumed, u32* n_records, u32* malformed); dbuf<u8> bam_buf, bam_buf_next;
+	// the record loop of the ingest (records.cu): the record store across chunks, then the replay by key into the fragment pools
+	void records_begin(const u16* tid_to_contig, u32 n_tid, const u8* interesting, const u8* viral, const u64* n_windows, u32 n_contigs, u32 max_itd_length, bool external_duplicate_marking, u64 expected_bytes);
+	void records_chunk(const u8* chunk, u64 bytes, u64 first, u64 chunk_pos, u64* n_records, u64* carry, u32* malformed, u64* error);
+	void records_finish(u16* const* coverage, u8* const* starts, u8* const* ends, u64* counters, u64* error);
+	dbuf<u8> rec_arena, rec_sa, rec_interesting, rec_viral, rec_cov_starts, rec_cov_ends; dbuf<u64> rec_at, rec_pos, rec_error, rec_counters, rec_cov_off; dbuf<i64> rec_hit;
+	dbuf<u32> rec_hash_lo, rec_hash_hi, rec_cov_words, rec_cov_n; dbuf<u16> rec_tid;
+	u64 rec_n, rec_arena_used, rec_carry, rec_carry_at, rec_expected_bytes, rec_cov_windows, rec_hash_mask; u32 rec_n_tid, rec_n_contigs, rec_max_itd; bool rec_external_dup, rec_open;
+	std::vector<u8> rec_error_record; // the body of the record a chunk's error names
 	// rows of the discarded-fusions file (rows.cu)
 	void set_row_texts(const arb_row_texts& t); void format_discarded_rows(const u8* confidence, u64* n_rows, u64* n_bytes); void get_row_text(char* out);
 	dbuf<char> row_gene_name, row_gene_id, row_contig_name, row_filter_name, row_text; dbuf<u32> row_gene_name_off, row_gene_id_off, row_contig_name_off, row_filter_name_off; dbuf<i32> row_exon_prev, row_exon_next;

@@ -1,5 +1,5 @@
-// fragtable.cu -- the resident fragment table, built on the device from the pools of the ingest's workers (functors: fragtable_hd.h).
-// After the record loop the host copies every worker's pools up once (page-locked: at full PCIe speed); the device then
+// fragtable.cu -- the resident fragment table, built on the device from the fragment pools of the record replay (records.cu; functors: fragtable_hd.h).
+// The device
 //   1. normalises the slots of every fragment and rejects the malformed ones (one thread per fragment, the alignment chain walked in the pool),
 //   2. orders the kept fragments by name: stable LSD radix sort of (name word, fragment), 4-byte words from the last one any name has to the first,
 //   3. lays out the columns: exclusive scans of CIGAR operations, sequence units and name bytes in name order, then one thread per fragment writes them,
@@ -10,35 +10,8 @@
 
 namespace arb {
 
-void engine::fragment_pools_upload(const arb_fragment_pools* pools, u32 n_pools) {
-	if (n_pools == 0) throw arb_error("arb_fragment_pools_upload: no pools");
-	ex.sync(); // kernels of the previous sample may still read the buffers that are about to be overwritten
-	stage_timer t_h2d(ex);
-	std::vector<u64> base((size_t) FT_POOLS * (n_pools + 1), 0);
-	for (u32 w = 0; w < n_pools; ++w) {
-		const arb_fragment_pools& p = pools[w];
-		const u64 sizes[FT_POOLS] = {p.n_frags, p.n_alns, p.n_name_bytes, p.n_cigars, (p.n_seq_bytes + 15) & ~(u64) 15}; // every worker's sequences start 16-byte aligned
-		for (u32 k = 0; k < FT_POOLS; ++k) base[(size_t) k * (n_pools + 1) + w + 1] = base[(size_t) k * (n_pools + 1) + w] + sizes[k];
-	}
-	auto total = [&](u32 k) { return base[(size_t) k * (n_pools + 1) + n_pools]; };
-	if (total(FT_FRAGS) >= 0x50000000ull) throw arb_error("more than 2^30 fragments");
-	pool_frags.ensure(total(FT_FRAGS)); pool_alns.ensure(total(FT_ALNS)); pool_names.ensure(total(FT_NAMES)); pool_cigars.ensure(total(FT_CIGARS)); pool_seqs.ensure(total(FT_SEQS));
-	u64 bytes = 0;
-	for (u32 w = 0; w < n_pools; ++w) {
-		const arb_fragment_pools& p = pools[w];
-		auto at = [&](u32 k) { return base[(size_t) k * (n_pools + 1) + w]; };
-		pool_frags.upload_at(ex, p.frags, p.n_frags, at(FT_FRAGS)); pool_alns.upload_at(ex, p.alns, p.n_alns, at(FT_ALNS));
-		pool_names.upload_at(ex, p.names, p.n_name_bytes, at(FT_NAMES)); pool_cigars.upload_at(ex, p.cigars, p.n_cigars, at(FT_CIGARS)); pool_seqs.upload_at(ex, p.seqs, p.n_seq_bytes, at(FT_SEQS));
-		bytes += p.n_frags * sizeof(arb_pool_fragment) + p.n_alns * sizeof(arb_pool_alignment) + p.n_name_bytes + p.n_cigars * 4 + p.n_seq_bytes;
-	}
-	pool_base.upload(ex, base.data(), base.size());
-	pool_workers = n_pools;
-	timings.h2d_ms = t_h2d.stop(); // the copies are complete: the host may reuse the pools
-	timings.h2d_bytes = bytes;
-}
-
 void engine::fragment_table_build(u64 sizes[6]) {
-	if (pool_workers == 0) throw arb_error("arb_fragment_table_build without arb_fragment_pools_upload");
+	if (pool_workers == 0) throw arb_error("arb_fragment_table_build without arb_records_finish");
 	const u32 W = pool_workers;
 	std::vector<u64> base(pool_base.size()); pool_base.download(ex, base.data(), base.size());
 	const u32 N = (u32) base[FT_FRAGS * (W + 1) + W];

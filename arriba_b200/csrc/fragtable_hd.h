@@ -1,4 +1,4 @@
-// fragtable_hd.h -- the fragment table from the pools of the ingest's workers (fragtable.cu drives it; the CPU stand-in runs the same functors).
+// fragtable_hd.h -- the fragment table from the fragment pools the record replay writes (records.cu; fragtable.cu drives it; the CPU stand-in runs the same functors).
 //   ft_normalise : brings a fragment's alignments into the canonical slots or rejects it (read_chimeric_alignments.cpp:340-373 disjoin_split_read_segments,
 //                  :377-506 remove_malformed_alignments), without writing anything: the rewritten CIGAR operations are kept as overrides of the pool's,
 //   ft_keep_fn   : one thread per fragment of the pools: kept or not, its CIGAR operations, sequence units and name length,

@@ -39,7 +39,7 @@ static void tune_allocator() { // once per process, also when two threads create
 	(void) done;
 }
 
-void arb_release_host_memory(void) { arb::host::host_block_trim(); arb::host::release_worker_cache(); }
+void arb_release_host_memory(void) { arb::host::host_block_trim(); }
 
 int arb_pipeline_create(arb_pipeline** out, const arb_run_options* o) {
 	tune_allocator();

@@ -1,4 +1,4 @@
-// ingest.h -- chimeric BAM ingest: BGZF/BAM decoding on host threads into structure-of-arrays fragment columns
+// ingest.h -- chimeric BAM ingest: BGZF inflate on host threads, the record loop on the device, into structure-of-arrays fragment columns
 // (arb_soa_chunk layout, fragments in name order), plus the by-products the later stages need (mapped read count,
 // coverage windows). Behavioural contract: read_chimeric_alignments (read_chimeric_alignments.cpp:560-773) and helpers
 // (:19-558), mark_multimappers (:792-802), coverage_t (read_stats.cpp:148-306). Only STAR "WithinBAM" input (-x) is
@@ -10,6 +10,7 @@
 #include <memory>
 #include <utility>
 #include <new>
+#include <functional>
 #include "refdata.h"
 struct arb_ctx;
 
@@ -28,7 +29,6 @@ struct coverage_windows { // 20 bp windows (read_stats.hpp:14)
 // them), and a process that runs sample after sample would pay it for gigabytes of columns every time. Blocks of 1 MiB and more go back to a free list per
 // size class (steps of 25 %) instead of the C library; host_block_trim() (arb_release_host_memory) hands them to the system.
 void* host_block_get(size_t bytes, size_t& granted);
-void release_worker_cache(); // the ingest keeps the workers' pools of a finished sample for the next one (ingest.cpp)
 void host_block_put(void* p, size_t granted);
 void host_block_trim();
 // where fresh blocks come from (default: malloc). The CUDA library installs page-locked blocks on 2 MiB pages (capi.cu); a NULL result falls back to malloc.
@@ -75,7 +75,11 @@ struct ingest_stats {
 	double t_inflate, t_parse, t_finalize;
 };
 
-struct ingest_options { bool external_duplicate_marking; u32 max_itd_length; std::string interesting_contigs, viral_contigs; int threads; struct ::arb_ctx* scan_ctx /* device context that finds the records of every chunk (arb_bam_scan) */; };
+struct ingest_options {
+	bool external_duplicate_marking; u32 max_itd_length; std::string interesting_contigs, viral_contigs; int threads /* inflate */;
+	struct ::arb_ctx* scan_ctx; // device context that runs the record loop and builds the fragment table
+	std::function<void()> after_header; // once the BAM header has grown the contig table: the contigs and the gene index must reach scan_ctx before the records
+};
 
 // reads the BAM, fills `out` (name order, slots normalised, multimappers marked); throws std::runtime_error on fatal input errors
 void read_chimeric_alignments(const std::string& bam_path, refdata& ref, const ingest_options& opt, fragment_table& out, coverage_windows& coverage, ingest_stats& stats);

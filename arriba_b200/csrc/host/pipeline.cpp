@@ -49,6 +49,7 @@ void pipeline::ingest() {
 	ingest_options io; io.external_duplicate_marking = opt.params.external_duplicate_marking; io.max_itd_length = opt.params.max_itd_length;
 	io.interesting_contigs = opt.interesting_contigs; io.viral_contigs = opt.viral_contigs; io.threads = threads;
 	attach_device(); io.scan_ctx = ctx;
+	io.after_header = [this]() { begin_upload(); send_annotation(); }; // the read-through test queries the GTF's genes (before the dummy genes of annotate())
 	read_chimeric_alignments(opt.bam_file, ref, io, frags, coverage, istats);
 	std::ostringstream s; s << "Reading chimeric alignments from '" << opt.bam_file << "' (total=" << frags.n << ")";
 	say(s.str());

@@ -108,34 +108,39 @@ int arb_push_chunk(arb_ctx* ctx, const arb_soa_chunk* chunk); /* H2D copy; repla
  * are page-locked; the whole-run driver builds them in page-locked blocks (registered with cudaHostRegister, recycled across samples). */
 int arb_push_chunk_begin(arb_ctx* ctx, const arb_soa_chunk* chunk);
 int arb_push_chunk_end(arb_ctx* ctx, const arb_soa_chunk* chunk);
-/* ---- BAM records of an inflated chunk -------------------------------------------------------------------------
- * The bookkeeping the reference's record loop (source/read_chimeric_alignments.cpp:611, sam_read1) does implicitly: where the records of a chunk of inflated
- * BGZF payload start (SAMv1 4.2: every record begins with its block_size) and which worker parses which record -- lists by read-name hash (FNV-1a), so that
- * the records of a fragment meet in one list; file order is kept inside a list. chunk: page-locked host memory makes the copy asynchronous; first = offset of
- * the first record; n_ref = reference sequences of the BAM header (sanity of guessed record starts); consumed = offset behind the last complete record;
- * record_offsets: capacity bytes / 36 + 1; malformed != 0: a block_size < 33 was met where a one-thread walk would have met it. */
-int arb_bam_scan(arb_ctx* ctx, const uint8_t* chunk, uint64_t bytes, uint64_t first, int32_t n_ref, uint32_t n_lists, uint64_t* consumed, uint32_t* n_records,
-                 uint32_t* list_begin /* n_lists + 1 */, uint32_t* record_offsets, uint32_t* malformed);
-/* ---- fragment table from the pools of the ingest's workers ---------------------------------------------------------
- * What the record loop of ingest leaves per worker: fragments (name, chain of alignments in arrival order) and pools of names, CIGAR operations and nt16
- * sequences. Offsets and links are local to the worker. The device turns the pools of all workers into the resident fragment table: slot normalisation and
- * rejection of malformed fragments (source/read_chimeric_alignments.cpp:340-506), name order (std::string::compare of "<qname>,<HI>[ITD]"), the SoA columns
- * in the layout arb_push_chunk takes (sequences back to back in fragment order, slot 0 then slot 1) and the multimapper flags (:792-802).
- *   arb_fragment_pools_upload : copies the pools (page-locked memory: at full PCIe speed) and returns when they are resident,
+/* ---- the record loop of the ingest ---------------------------------------------------------------------------------
+ * What the reference's record loop does (source/read_chimeric_alignments.cpp:611-749, -x input), on the device. The host inflates the BGZF blocks and reads
+ * the BAM header; the device finds the records of every chunk, keeps what the loop needs of them (a record store that lives across chunks: mates and
+ * supplementaries of one read may sit anywhere in the file), then groups them by "<qname>,<HI>" and replays the loop in file order into the fragment pools.
+ *   arb_records_begin  : tid_to_contig = contig id of every BAM reference (n_tid); interesting / viral contig flags and the number of 20-bp coverage windows
+ *                        per contig (n_contigs = the contigs of arb_set_contigs, which must have been called with the grown table; the gene index of
+ *                        arb_set_annotation is the one the read-through test queries); expected_bytes = the inflated size of the file (sizes the store),
+ *   arb_records_chunk  : one chunk of inflated payload (page-locked host memory makes the copy asynchronous). chunk_pos = its position in the inflated
+ *                        stream; first = offset of the first record (behind the header) in the first chunk, else 0. The unfinished record at the end of a
+ *                        chunk is kept on the device for the next one: carry = its bytes (not 0 after the last chunk: truncated file). malformed != 0:
+ *                        a block_size < 33 where a one-thread walk would meet it. error = (file position << 3 | kind) of the first fatal record error so
+ *                        far, ~0 for none (kinds: 1 unreadable record, 2 CIGAR does not fit the sequence, 3 alignment beyond its contig, 4 too many
+ *                        overlapping annotation records at one locus),
+ *   arb_records_error_record : the record body (after block_size) an error of kinds 1-3 names,
+ *   arb_records_finish : the replay; coverage / starts / ends = per contig caller-allocated windows (the counts of arb_records_begin), counters = mapped
+ *                        reads, malformed supplementaries, secondaries without HI, 1 if any split read or discordant mate was seen, then the pristine reads
+ *                        of every contig (4 + n_contigs); error as above. On success the fragment pools are ready for arb_fragment_table_build.
+ * ---- fragment table from the pools ---------------------------------------------------------------------------------------------------------------
+ * The pools: fragments (name, chain of alignments in the loop's order) and pools of names, CIGAR operations and nt16 sequences. The device turns them into
+ * the resident fragment table: slot normalisation and rejection of malformed fragments (source/read_chimeric_alignments.cpp:340-506), name order
+ * (std::string::compare of "<qname>,<HI>[ITD]"), the SoA columns in the layout arb_push_chunk takes (sequences back to back in fragment order, slot 0 then
+ * slot 1) and the multimapper flags (:792-802).
  *   arb_fragment_table_build  : builds the table, which becomes the resident one (as after arb_push_chunk_begin); sizes = {fragments, rejected fragments,
  *                               CIGAR operations, sequence bytes, name bytes, neighbours in name order with the same read name (mark_multimappers' count)},
  *   arb_fragment_table_download : the host copy (caller-allocated: n, n, n, 3n; 3n, 3n, 3n, 3n, 3n; 2n, 2n; 3n, 3n; CIGAR operations + 1, sequence bytes;
  *                               name bytes, n + 1 offsets). */
 typedef struct { uint8_t supplementary, first_in_pair, forward; uint16_t contig; int32_t start, end; uint32_t cigar_off, cigar_cnt; uint64_t seq_off; uint32_t seq_len; int32_t next; } arb_pool_alignment;
 typedef struct { uint64_t name_off; uint32_t name_len; int32_t head, tail; uint32_t count; uint8_t single_end, duplicate; } arb_pool_fragment;
-typedef struct {
-	const arb_pool_fragment* frags; uint64_t n_frags;
-	const arb_pool_alignment* alns; uint64_t n_alns;   /* `next` links a fragment's alignments, -1 ends the chain */
-	const char* names; uint64_t n_name_bytes;
-	const uint32_t* cigars; uint64_t n_cigars;
-	const uint8_t* seqs; uint64_t n_seq_bytes;         /* each sequence 16-byte aligned */
-} arb_fragment_pools;
-int arb_fragment_pools_upload(arb_ctx* ctx, const arb_fragment_pools* pools, uint32_t n_pools);
+int arb_records_begin(arb_ctx* ctx, const uint16_t* tid_to_contig, uint32_t n_tid, const uint8_t* interesting, const uint8_t* viral, const uint64_t* n_windows, uint32_t n_contigs,
+                      uint32_t max_itd_length, int external_duplicate_marking, uint64_t expected_bytes);
+int arb_records_chunk(arb_ctx* ctx, const uint8_t* chunk, uint64_t bytes, uint64_t first, uint64_t chunk_pos, uint64_t* n_records, uint64_t* carry, uint32_t* malformed, uint64_t* error);
+int arb_records_error_record(arb_ctx* ctx, const uint8_t** body, uint64_t* bytes);
+int arb_records_finish(arb_ctx* ctx, uint16_t* const* coverage, uint8_t* const* starts, uint8_t* const* ends, uint64_t* counters, uint64_t* error);
 int arb_fragment_table_build(arb_ctx* ctx, uint64_t sizes[6]);
 int arb_fragment_table_download(arb_ctx* ctx, const arb_soa_chunk* columns, char* names, uint64_t* name_off);
 /* ---- annotation of the resident fragments -------------------------------------------------------------------
@@ -369,7 +374,7 @@ typedef struct arb_timings {
 	float order_ms;             /* arb_replay_insertion_order */
 	float partners_ms;          /* arb_partner_counts */
 	float rows_ms;              /* arb_format_discarded_rows */
-	float bam_scan_ms;          /* arb_bam_scan, summed over the chunks of the last sample (copy + kernels + lists back) */
+	float bam_scan_ms;          /* the record loop of the last sample: arb_records_chunk over all chunks (copy + kernels) and arb_records_finish */
 	float consensus_ms;         /* arb_build_consensus, summed over the batches of the last sample */
 	uint64_t mismapper_algorithmic_bytes; /* SURVEY.md section 8(d) budget of pass 1 of the re-alignment: per searched sequence of length l, 3l/8 + 8(l-8) + 4*hits + l/2 */
 	uint64_t mismapper_sequences, mismapper_hits; /* sequences searched by pass 1 (segment x gene x strand) and k-mer hits they visited */
