@@ -6,7 +6,10 @@
 // only stops it from being tested again, and the test reads nothing the loop writes: the verdict is "eligible and some rule that shares a bin with the
 // candidate matches", whatever the order of the file or of the candidates. Here the rules' bins become (contig, bin) keys, sorted into a key table with one
 // rule list per key; every eligible candidate looks up its own bins and tests the rules listed there.
-// The rule columns and rule_match do not depend on the blacklist: a file of known fusions (-k) has the same format and the same item test.
+// The files of known fusions (-k, recover_known_fusions.cpp:14-100) and of tags (-t, annotate_tags.cpp) have the same format and the same item test. They
+// differ in three ways: the rules' bins are not widened by max_mate_gap; the match is directional (item 1 against the 5' side, item 2 against the 3' side,
+// known fusions also swapped when the transcript start is ambiguous and the breakpoints are far apart); and a tag needs every matching rule, not just one.
+// So the rule columns, the key table, the candidate's bins and the item test are shared by three searches, each with its own set of rules.
 #pragma once
 #include "model.h"
 #include "prims.h"        // append_slot
@@ -14,6 +17,7 @@
 #include "../../include/arriba_b200.h" // ARB_RULE_*
 #include "events_hd.h"    // cand_state
 #include "genomic_hd.h"   // wrap_add / wrap_sub
+#include <climits>
 
 namespace arb {
 
@@ -34,11 +38,17 @@ ARB_HD void rule_bins(i64 start, i64 end, i32& lo, i32& hi) {
 	if (b > RULE_BIN_LIMIT) b = RULE_BIN_LIMIT;
 	lo = (i32) a; hi = (i32) b; // lo > hi: no bins
 }
+// the same for int coordinates (every candidate range), in 32-bit arithmetic: a 64-bit division is a called subroutine on the device
+ARB_HD void rule_bins32(i32 start, i32 end, i32& lo, i32& hi) {
+	lo = start / (i32) RULE_BIN_SIZE;
+	hi = end <= INT_MAX - 99999 ? (end + 99999) / (i32) RULE_BIN_SIZE : end / (i32) RULE_BIN_SIZE + (end % (i32) RULE_BIN_SIZE != 0);
+}
 ARB_HD u32 rule_bin_key(u32 contig, i32 bin) { return contig << 16 | (u32) (bin + 32768); }
 
-// the bins a positional item of a rule is looked up under: (contig, start - max_mate_gap, end + max_mate_gap) (:272-275)
-ARB_HD void rule_item_bins(const rule_columns& r, u32 rule, u32 side, i32 max_mate_gap, i32& lo, i32& hi) {
-	rule_bins((i64) r.start[side][rule] - max_mate_gap, (i64) r.end[side][rule] + max_mate_gap, lo, hi);
+// the bins a positional item of a rule is looked up under: (contig, start - widen, end + widen); widen is max_mate_gap for the blacklist (:272-275) and 0 for
+// known fusions and tags (recover_known_fusions.cpp:32-34, annotate_tags.cpp:36-38)
+ARB_HD void rule_item_bins(const rule_columns& r, u32 rule, u32 side, i32 widen, i32& lo, i32& hi) {
+	rule_bins((i64) r.start[side][rule] - widen, (i64) r.end[side][rule] + widen, lo, hi);
 }
 
 // overlapping_fraction (:123-135): the quotient in double, returned as float; the four branches as written (the second has no "+ 1")
@@ -96,16 +106,21 @@ struct rule_match {
 	ARB_HD bool operator()(u32 rule, u32 k) const { // both orders of the two items (:280-283)
 		return (item(rule, 0, k, 1) && item(rule, 1, k, 2)) || (item(rule, 0, k, 2) && item(rule, 1, k, 1));
 	}
+	// item 1 against the 5' side and item 2 against the 3' side (recover_known_fusions.cpp:65-68, annotate_tags.cpp:62-65); swapped: the other way round
+	ARB_HD bool directional(u32 rule, u32 k, bool swapped) const {
+		const u32 g5 = (c.bits[k] & CB_TSTART_GENE1) ? 1 : 2, g3 = 3 - g5;
+		return swapped ? item(rule, 0, k, g3) && item(rule, 1, k, g5) : item(rule, 0, k, g5) && item(rule, 1, k, g3);
+	}
 };
 
-// ---- key table of the rules (engine: filter_blacklist): counts, scan, fill, sort, then one entry per distinct key
+// ---- key table of the rules (blacklist.cu: build_rule_keys): counts, scan, fill, sort, then one entry per distinct key
 struct rule_key_count_fn { // number of (contig, bin) keys of every rule
-	rule_columns r; i32 max_mate_gap; u32* count; unsigned long long* total;
+	rule_columns r; i32 widen; u32* count; unsigned long long* total;
 	ARB_HD void operator()(u32 rule) const {
 		u32 n = 0;
 		for (u32 side = 0; side < 2; ++side) {
 			if (!rule_item_positional(r.type[side][rule])) continue;
-			i32 lo, hi; rule_item_bins(r, rule, side, max_mate_gap, lo, hi);
+			i32 lo, hi; rule_item_bins(r, rule, side, widen, lo, hi);
 			if (hi >= lo) n += (u32) (hi - lo + 1);
 		}
 		count[rule] = n;
@@ -117,12 +132,12 @@ struct rule_key_count_fn { // number of (contig, bin) keys of every rule
 	}
 };
 struct rule_key_fill_fn { // the keys of rule `rule` at its offset, the rule as their value
-	rule_columns r; i32 max_mate_gap; const u32* offset; u32* key; u32* rule_of;
+	rule_columns r; i32 widen; const u32* offset; u32* key; u32* rule_of;
 	ARB_HD void operator()(u32 rule) const {
 		u32 at = offset[rule];
 		for (u32 side = 0; side < 2; ++side) {
 			if (!rule_item_positional(r.type[side][rule])) continue;
-			i32 lo, hi; rule_item_bins(r, rule, side, max_mate_gap, lo, hi);
+			i32 lo, hi; rule_item_bins(r, rule, side, widen, lo, hi);
 			for (i32 b = lo; b <= hi; ++b) { key[at] = rule_bin_key(r.contig[side][rule], b); rule_of[at] = rule; ++at; }
 		}
 	}
@@ -153,58 +168,175 @@ struct rule_key_table {
 	}
 };
 
-// ---- the search: one thread per eligible candidate; a candidate with a long rule list goes to a group of lanes
-struct blacklist_search {
-	rule_match m; rule_key_table t;
-	const u32* ids; u8* verdict;        // eligible candidates, one verdict byte each
-	u32 short_list;                     // lists up to this length are walked by the candidate's own thread
-	u32* heavy; u32* n_heavy;           // positions in `ids` of the candidates queued for a group of lanes
-
-	// the four ranges a candidate is indexed under (:244-247): both breakpoints, then both genes
+// ---- the rule lists a candidate meets: the bins of its four ranges, each distinct bin once
+struct cand_bins {
+	cand_state c; annot_view an; rule_key_table t;
+	// the four ranges a candidate is indexed under (:244-247, recover_known_fusions.cpp:53-57, annotate_tags.cpp:48-52): both breakpoints, then both genes
 	ARB_HD void range(u32 k, u32 x, u32& contig, i32& lo, i32& hi) const {
-		const cand_state& c = m.c;
 		contig = (x & 1) ? c.contig2[k] : c.contig1[k];
-		if (x < 2) { const i32 bp = x ? c.bp2[k] : c.bp1[k]; rule_bins(bp, bp, lo, hi); }
-		else { const u32 g = x == 2 ? c.gene1[k] : c.gene2[k]; rule_bins(m.an.gene_start[g], m.an.gene_end[g], lo, hi); }
+		if (x < 2) { const i32 bp = x ? c.bp2[k] : c.bp1[k]; rule_bins32(bp, bp, lo, hi); }
+		else { const u32 g = x == 2 ? c.gene1[k] : c.gene2[k]; rule_bins32(an.gene_start[g], an.gene_end[g], lo, hi); }
 	}
-	// a bin already listed by an earlier range of the same candidate is looked up once
+	// a bin already listed by an earlier range of the same candidate is looked up once (every search's verdict is the same either way)
 	ARB_HD bool listed_before(u32 k, u32 x, u32 contig, i32 bin) const {
 		for (u32 y = 0; y < x; ++y) { u32 cy; i32 lo, hi; range(k, y, cy, lo, hi); if (cy == contig && bin >= lo && bin <= hi) return true; }
 		return false;
 	}
-	// lane `lane` of `lanes` tests rules lo + lane, lo + lane + lanes, ... of every list of candidate k; a single thread is lane 0 of 1
-	ARB_HD bool lane_walk(u32 k, u32 lane, u32 lanes) const {
+	// v(a, e) for the rule list rules[a .. e) of every distinct bin of candidate k, until v returns true; returns whether it did
+	template <class V> ARB_HD bool visit(u32 k, V& v) const {
 		for (u32 x = 0; x < 4; ++x) {
 			u32 contig; i32 lo, hi; range(k, x, contig, lo, hi);
 			for (i32 b = lo; b <= hi; ++b) {
 				u32 a, e;
 				if (listed_before(k, x, contig, b) || !t.find(rule_bin_key(contig, b), a, e)) continue;
-				for (u32 q = a + lane; q < e; q += lanes) if (m(t.rules[q], k)) return true;
+				if (v(a, e)) return true;
 			}
 		}
 		return false;
 	}
+};
+
+// ---- "does some listed rule pass Test": one thread per candidate id; a candidate with a long rule list goes to a group of lanes
+// Test: ARB_HD bool operator()(u32 rule, u32 k)
+template <class Test> struct rule_search {
+	cand_bins b; Test test;
+	const u32* ids; u8* verdict;        // candidates, one verdict byte each
+	u32 short_list;                     // lists up to this length are walked by the candidate's own thread
+	u32* heavy; u32* n_heavy;           // positions in `ids` of the candidates queued for a group of lanes
+
+	struct lanes_fn { // lane `lane` of `lanes` tests rules a + lane, a + lane + lanes, ... of a list
+		const rule_search* s; u32 k, lane, lanes;
+		ARB_HD bool operator()(u32 a, u32 e) const { for (u32 q = a + lane; q < e; q += lanes) if (s->test(s->b.t.rules[q], k)) return true; return false; }
+	};
+	struct thread_fn { // the whole list, or 2 when it is too long for one thread
+		const rule_search* s; u32 k; u32 result;
+		ARB_HD bool operator()(u32 a, u32 e) {
+			if (e - a > s->short_list) { result = 2; return true; }
+			for (u32 q = a; q < e; ++q) if (s->test(s->b.t.rules[q], k)) { result = 1; return true; }
+			return false;
+		}
+	};
+	// a single thread is lane 0 of 1
+	ARB_HD bool lane_walk(u32 k, u32 lane, u32 lanes) const { lanes_fn v = {this, k, lane, lanes}; return b.visit(k, v); }
+	ARB_HD void operator()(u32 i) const {
+		thread_fn v = {this, ids[i], 0};
+		b.visit(ids[i], v);
+		if (v.result == 2) heavy[append_slot(n_heavy)] = i;
+		else verdict[i] = (u8) v.result;
+	}
+};
+
+typedef rule_search<rule_match> blacklist_search;
+
+// ---- known fusions (recover_known_fusions.cpp:41-92): a rule rescues an eligible candidate if it matches it directionally (or swapped, when the transcript
+// start is ambiguous and the breakpoints are not within 1 Mb on one contig), and either both of its items are positions or the candidate is well supported:
+// >= 2 reads, or both breakpoints spliced with coverage < 200 at them, on different contigs or more than 1 Mb apart. The rules are read in order, but the
+// outcome is a plain "some rule rescues it".
+ARB_HD i64 abs_i64(i64 a) { return a < 0 ? -a : a; }
+ARB_HD bool cand_close(const cand_state& c, u32 k) { return c.contig1[k] == c.contig2[k] && abs_i64((i64) c.bp2[k] - c.bp1[k]) < 1000000; }
+// the per-candidate half of the rescue condition (:81-85), computed once per eligible candidate before the search: indexed by candidate id
+struct known_support_fn {
+	cand_state c; annot_view an; coverage_view cov; const u32* ids; u8* supported;
 	ARB_HD void operator()(u32 i) const {
 		const u32 k = ids[i];
-		for (u32 x = 0; x < 4; ++x) {
-			u32 contig; i32 lo, hi; range(k, x, contig, lo, hi);
-			for (i32 b = lo; b <= hi; ++b) {
-				u32 a, e;
-				if (listed_before(k, x, contig, b) || !t.find(rule_bin_key(contig, b), a, e)) continue;
-				if (e - a > short_list) { heavy[append_slot(n_heavy)] = i; return; }
-				for (u32 q = a; q < e; ++q) if (m(t.rules[q], k)) { verdict[i] = 1; return; }
-			}
+		bool ok = cand_support(c, k) >= 2;
+		if (!ok && cand_both_spliced(c, an, k)) {
+			const int cov1 = cov.get(c.contig1[k], c.bp1[k], c.dir1[k] == UPSTREAM ? DOWNSTREAM : UPSTREAM), cov2 = cov.get(c.contig2[k], c.bp2[k], c.dir2[k] == UPSTREAM ? DOWNSTREAM : UPSTREAM);
+			ok = cov1 + cov2 < 200 && (c.contig1[k] != c.contig2[k] || abs_i64((i64) c.bp2[k] - c.bp1[k]) > 1000000);
 		}
-		verdict[i] = 0;
+		supported[k] = ok ? 1 : 0;
 	}
+};
+struct known_fusion_test {
+	rule_match m; const u8* supported;
+	ARB_HD bool operator()(u32 rule, u32 k) const {
+		if (!supported[k] && !(m.r.type[0][rule] == ARB_RULE_POSITION && m.r.type[1][rule] == ARB_RULE_POSITION)) return false; // a match would not rescue
+		const u32 orders = m.c.bits2[k] && !cand_close(m.c, k) ? 2 : 1; // the swapped order only for an ambiguous transcript start, breakpoints not within 1 Mb
+		for (u32 o = 0; o < orders; ++o) if (m.directional(rule, k, o != 0)) return true;
+		return false;
+	}
+};
+typedef rule_search<known_fusion_test> known_fusion_search;
+
+// ---- tags (annotate_tags.cpp:45-83): the ranks of the tags of every rule that matches a row directionally. Pass 1 counts them per row, pass 2 (offset set)
+// writes (rank, candidate) pairs at the row's offset. Duplicates (a rule listed under two bins of the row, two rules with one tag) are removed afterwards.
+struct tag_search {
+	cand_bins b; rule_match m; const u32* rank; // rank of every rule's tag among the distinct tags in bytewise order
+	const u32* ids; u32 short_list;
+	u8* heavy_mark; u32* heavy; u32* n_heavy;   // pass 1 queues the rows with a long list; pass 2 leaves them to the lane groups as well
+	u32* count; const u32* offset;              // pass 1 writes count, pass 2 reads offset
+	unsigned long long* total;                  // pass 1: the sum of all counts, in 64 bits (the 32-bit offsets are used only once it is known to fit)
+	u32* out_rank; u32* out_cand;
+
+	struct lanes_fn { // lane `lane` of `lanes`: rules a + lane, a + lane + lanes, ...; pass 2 writes at `at`, which advances
+		const tag_search* s; u32 k, lane, lanes, n; u32 at;
+		ARB_HD bool operator()(u32 a, u32 e) {
+			for (u32 q = a + lane; q < e; q += lanes) {
+				const u32 rule = s->b.t.rules[q];
+				if (!s->m.directional(rule, k, false)) continue;
+				if (s->offset) { s->out_rank[at] = s->rank[rule]; s->out_cand[at] = k; ++at; }
+				++n;
+			}
+			return false;
+		}
+	};
+	struct long_fn { const tag_search* s; ARB_HD bool operator()(u32 a, u32 e) const { return e - a > s->short_list; } };
+	// a single thread is lane 0 of 1; returns the number of matches of this lane
+	ARB_HD u32 lane_walk(u32 k, u32 lane, u32 lanes, u32 at) const { lanes_fn v = {this, k, lane, lanes, 0, at}; b.visit(k, v); return v.n; }
+	ARB_HD void operator()(u32 i) const {
+		const u32 k = ids[i];
+		if (offset) { if (!heavy_mark[i]) lane_walk(k, 0, 1, offset[i]); return; }
+		long_fn l = {this};
+		if (b.visit(k, l)) { heavy_mark[i] = 1; count[i] = 0; heavy[append_slot(n_heavy)] = i; return; }
+		heavy_mark[i] = 0; count[i] = lane_walk(k, 0, 1, 0);
+		add_total(count[i]);
+	}
+	ARB_HD void add_total(u32 n) const {
+		if (!n) return;
+#ifdef __CUDA_ARCH__
+		atomicAdd(total, (unsigned long long) n);
+#else
+		*total += n;
+#endif
+	}
+};
+
+// the distinct (candidate, rank) pairs after the sort by (candidate, rank): a pair is kept if it differs from the one before it
+struct tag_head_fn {
+	const u32* cand; const u32* rank; u32* head;
+	ARB_HD void operator()(u32 j) const { head[j] = j == 0 || cand[j] != cand[j - 1] || rank[j] != rank[j - 1]; }
+};
+struct tag_compact_fn { // pair j -> slot[j] of the CSR, and one more tag for its candidate
+	const u32* cand; const u32* rank; const u32* head; const u32* slot; u32* csr_rank; u32* per_cand;
+	ARB_HD void operator()(u32 j) const { if (head[j]) { csr_rank[slot[j]] = rank[j]; atomic_add_u32(&per_cand[cand[j]], 1); } }
 };
 
 #ifdef ARB_DEVICE_BUILD
 // a group of lanes per queued candidate: every lane tests its share of every list, __any_sync combines them
-__device__ inline void blacklist_group(const lane_group& g, const blacklist_search& s, u32 i) {
+template <class Test> __device__ inline void rule_search_group(const lane_group& g, const rule_search<Test>& s, u32 i) {
 	const bool found = s.lane_walk(s.ids[i], g.lane, g.lanes);
 	const bool any = __any_sync(g.mask, found);
 	if (g.lane == 0) s.verdict[i] = any ? 1 : 0;
+}
+// a group of lanes per queued row: every lane tests its share of a list, the ballot counts the matches and gives every lane its write position
+struct tag_group_fn {
+	const tag_search* s; const lane_group* g; u32 k, n, at;
+	__device__ bool operator()(u32 a, u32 e) {
+		for (u32 base = a; base < e; base += g->lanes) {
+			const u32 q = base + g->lane;
+			const u32 rule = q < e ? s->b.t.rules[q] : 0;
+			const bool hit = q < e && s->m.directional(rule, k, false);
+			const u32 mask = __ballot_sync(g->mask, hit);
+			if (hit && s->offset) { const u32 j = at + n + __popc(mask & ((1u << g->lane) - 1u)); s->out_rank[j] = s->rank[rule]; s->out_cand[j] = k; }
+			n += __popc(mask);
+		}
+		return false;
+	}
+};
+__device__ inline void tag_group(const lane_group& g, const tag_search& s, u32 i) {
+	tag_group_fn v = {&s, &g, s.ids[i], 0, s.offset ? s.offset[i] : 0};
+	s.b.visit(v.k, v);
+	if (!s.offset && g.lane == 0) { s.count[i] = v.n; s.add_total(v.n); }
 }
 #endif
 

@@ -188,11 +188,27 @@ int arb_mark_genomic_support(arb_ctx* ctx, int32_t max_distance, int32_t max_itd
 int arb_get_genomic_support(arb_ctx* ctx, int32_t* closest1, int32_t* closest2) { ARB_API_BEGIN(ctx) ctx->e.get_genomic_support(closest1, closest2); ARB_API_END(ctx) }
 int arb_set_blacklist(arb_ctx* ctx, uint32_t n, const uint8_t* t1, const uint8_t* t2, const uint8_t* s1, const uint8_t* s2, const uint16_t* c1, const uint16_t* c2,
                       const int32_t* b1, const int32_t* e1, const int32_t* b2, const int32_t* e2, const uint32_t* g1, const uint32_t* g2) {
-	ARB_API_BEGIN(ctx) ctx->e.set_blacklist(n, t1, t2, s1, s2, c1, c2, b1, e1, b2, e2, g1, g2); ARB_API_END(ctx)
+	ARB_API_BEGIN(ctx) ctx->e.set_rules(ctx->e.blacklist_rules, "arb_set_blacklist", n, t1, t2, s1, s2, c1, c2, b1, e1, b2, e2, g1, g2); ARB_API_END(ctx)
 }
 int arb_filter_blacklist(arb_ctx* ctx, uint32_t n_ids, const uint32_t* ids, float evalue_cutoff, int32_t max_mate_gap, uint8_t* verdicts, uint32_t* n_blacklisted) {
 	ARB_API_BEGIN(ctx) const uint32_t b = ctx->e.filter_blacklist(n_ids, ids, evalue_cutoff, max_mate_gap, verdicts); if (n_blacklisted) *n_blacklisted = b; ARB_API_END(ctx)
 }
+int arb_set_known_fusions(arb_ctx* ctx, uint32_t n, const uint8_t* t1, const uint8_t* t2, const uint8_t* s1, const uint8_t* s2, const uint16_t* c1, const uint16_t* c2,
+                          const int32_t* b1, const int32_t* e1, const int32_t* b2, const int32_t* e2, const uint32_t* g1, const uint32_t* g2) {
+	ARB_API_BEGIN(ctx) ctx->e.set_rules(ctx->e.known_rules, "arb_set_known_fusions", n, t1, t2, s1, s2, c1, c2, b1, e1, b2, e2, g1, g2); ARB_API_END(ctx)
+}
+int arb_recover_known_fusions(arb_ctx* ctx, uint32_t n_ids, const uint32_t* ids, int32_t max_mate_gap, uint8_t* verdicts, uint32_t* n_rescued) {
+	ARB_API_BEGIN(ctx) const uint32_t r = ctx->e.recover_known_fusions(n_ids, ids, max_mate_gap, verdicts); if (n_rescued) *n_rescued = r; ARB_API_END(ctx)
+}
+int arb_set_tags(arb_ctx* ctx, uint32_t n, const uint8_t* t1, const uint8_t* t2, const uint8_t* s1, const uint8_t* s2, const uint16_t* c1, const uint16_t* c2,
+                 const int32_t* b1, const int32_t* e1, const int32_t* b2, const int32_t* e2, const uint32_t* g1, const uint32_t* g2,
+                 const uint32_t* tag_rank, uint32_t n_tags, const char* tag_chars, const uint32_t* tag_off) {
+	ARB_API_BEGIN(ctx) ctx->e.set_rules(ctx->e.tag_rules, "arb_set_tags", n, t1, t2, s1, s2, c1, c2, b1, e1, b2, e2, g1, g2); ctx->e.set_tags(tag_rank, n_tags, tag_chars, tag_off); ARB_API_END(ctx)
+}
+int arb_annotate_tags(arb_ctx* ctx, uint32_t n_ids, const uint32_t* ids, int32_t max_mate_gap, uint64_t* n_pairs) {
+	ARB_API_BEGIN(ctx) const uint64_t p = ctx->e.annotate_tags(n_ids, ids, max_mate_gap); if (n_pairs) *n_pairs = p; ARB_API_END(ctx)
+}
+int arb_get_tags(arb_ctx* ctx, uint32_t* off, uint32_t* ranks) { ARB_API_BEGIN(ctx) ctx->e.get_tags(off, ranks); ARB_API_END(ctx) }
 int arb_get_slot_swaps(arb_ctx* ctx, uint8_t* out) { ARB_API_BEGIN(ctx) ctx->e.get_slot_swaps(out); ARB_API_END(ctx) }
 
 } // extern "C"

@@ -14,7 +14,7 @@ void default_params(arb_params& p) { // options.cpp:71-107
 	p.max_mismapper_fraction = 0.8f; p.max_homolog_identity = 0.3f;
 }
 
-engine::engine(): row_max_itd_length(0), has_row_texts(false), row_text_bytes(0), kmer_block_shift(0), kmer_blocks(0), coverage_contigs(0), work_part(0), work_parts(1), mismap_items_total(0), mismap_ms_part(0), n_splice_sites(0), annot_pool_cap(0), n_dummy(0), n_gene_entries(0), push_cigar_ops(0), pool_workers(0), frag_name_bytes(0), rec_n(0), rec_arena_used(0), rec_carry(0), rec_carry_at(0), rec_expected_bytes(0), rec_cov_windows(0), rec_hash_mask(~(u64) 0), rec_n_tid(0), rec_n_contigs(0), rec_max_itd(0), rec_external_dup(false), rec_open(false), cascade_smem_bytes(0), cascade_resident_blocks(0), device(0), table_n(0), table_k(0), has_contigs(false), has_annotation(false), filters_done(false), merge_log_n(0), kmer_index_contigs(0), kmer_indexed(0), has_splice_sites(false), genomic_n(0), genomic_keys(0), genomic_heavy(0), has_genomic_breakpoints(false), blacklist_n(0), blacklist_heavy(0), has_blacklist(false) {
+engine::engine(): row_max_itd_length(0), has_row_texts(false), row_text_bytes(0), kmer_block_shift(0), kmer_blocks(0), coverage_contigs(0), work_part(0), work_parts(1), mismap_items_total(0), mismap_ms_part(0), n_splice_sites(0), annot_pool_cap(0), n_dummy(0), n_gene_entries(0), push_cigar_ops(0), pool_workers(0), frag_name_bytes(0), rec_n(0), rec_arena_used(0), rec_carry(0), rec_carry_at(0), rec_expected_bytes(0), rec_cov_windows(0), rec_hash_mask(~(u64) 0), rec_n_tid(0), rec_n_contigs(0), rec_max_itd(0), rec_external_dup(false), rec_open(false), cascade_smem_bytes(0), cascade_resident_blocks(0), device(0), table_n(0), table_k(0), has_contigs(false), has_annotation(false), filters_done(false), merge_log_n(0), kmer_index_contigs(0), kmer_indexed(0), has_splice_sites(false), genomic_n(0), genomic_keys(0), genomic_heavy(0), has_genomic_breakpoints(false), n_tags(0), tag_csr_n(0), tag_csr_pairs(0), has_tags(false), has_tag_csr(false), blacklist_heavy(0), known_heavy(0), tags_heavy(0) {
 	default_params(params);
 	memset(&timings, 0, sizeof(timings));
 	cons_rows = 0; cons_seq_bytes = cons_pos_count = cons_clip_bytes = 0;
@@ -200,7 +200,7 @@ void engine::adopt_table(const exec_ctx& cx, u64 n_cigar, u64 n_seq_bytes) {
 	push_alignments = st[2]; push_bases = st[1]; push_cigar_ops = n_cigar;
 	push_open = true;
 	filters_done = false;
-	cands.n = 0; cands.genomic_marked = false;
+	cands.n = 0; cands.genomic_marked = false; has_tag_csr = false;
 }
 
 void engine::push_chunk_end(const arb_soa_chunk& c) {

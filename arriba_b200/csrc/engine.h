@@ -184,12 +184,22 @@ public:
 	void set_genomic_breakpoints(u32 n, const u16* c1, const u16* c2, const u8* d1, const u8* d2, const i32* p1, const i32* p2);
 	u32 mark_genomic_support(i32 max_distance, i32 max_itd_length); void get_genomic_support(i32* closest1, i32* closest2);
 	dbuf<u64> genomic_key_table; dbuf<u32> genomic_key_begin; dbuf<i32> genomic_pos1, genomic_pos2; u32 genomic_n, genomic_keys, genomic_heavy; bool has_genomic_breakpoints;
-	// blacklist (blacklist.cu): the rule columns in file order; the key table is built per call, it depends on max_mate_gap
-	void set_blacklist(u32 n, const u8* type1, const u8* type2, const u8* strand1, const u8* strand2, const u16* contig1, const u16* contig2,
-	                   const i32* start1, const i32* end1, const i32* start2, const i32* end2, const u32* gene1, const u32* gene2);
+	// rules of a blacklist (-b), known fusions (-k) or tags (-t) file (blacklist.cu): the rule columns in file order; the key tables are built per call (the
+	// blacklist's depends on max_mate_gap)
+	struct rule_set {
+		dbuf<u8> type1, type2, strand1, strand2; dbuf<u16> contig1, contig2; dbuf<i32> start1, end1, start2, end2; dbuf<u32> gene1, gene2;
+		u32 n; bool loaded;
+		rule_set(): n(0), loaded(false) {}
+	};
+	void set_rules(rule_set& set, const char* who, u32 n, const u8* type1, const u8* type2, const u8* strand1, const u8* strand2, const u16* contig1, const u16* contig2,
+	               const i32* start1, const i32* end1, const i32* start2, const i32* end2, const u32* gene1, const u32* gene2);
+	rule_set blacklist_rules, known_rules, tag_rules;
 	u32 filter_blacklist(u32 n_ids, const u32* ids, float evalue_cutoff, i32 max_mate_gap, u8* verdicts);
-	dbuf<u8> bl_type1, bl_type2, bl_strand1, bl_strand2; dbuf<u16> bl_contig1, bl_contig2; dbuf<i32> bl_start1, bl_end1, bl_start2, bl_end2; dbuf<u32> bl_gene1, bl_gene2;
-	u32 blacklist_n, blacklist_heavy; bool has_blacklist;
+	u32 recover_known_fusions(u32 n_ids, const u32* ids, i32 max_mate_gap, u8* verdicts);
+	void set_tags(const u32* rank, u32 n_tags, const char* chars, const u32* off); // after set_rules(tag_rules, ...): the tag rank of every rule and the tag texts
+	u64 annotate_tags(u32 n_ids, const u32* ids, i32 max_mate_gap); void get_tags(u32* off, u32* ranks);
+	dbuf<u32> tag_rank_of_rule, tag_text_off, tag_csr_off, tag_csr_rank; dbuf<char> tag_text; u32 n_tags, tag_csr_n; u64 tag_csr_pairs; bool has_tags, has_tag_csr;
+	u32 blacklist_heavy, known_heavy, tags_heavy;
 private:
 	read_filter_params make_filter_params();
 	unsigned long genome_size() const;

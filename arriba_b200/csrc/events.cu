@@ -7,7 +7,7 @@ namespace arb {
 static cand_state make_state(cand_store& c, u32* n1, u32* n2) {
 	cand_state s;
 	s.n = c.n; s.gene1 = c.gene1.ptr(); s.gene2 = c.gene2.ptr(); s.contig1 = c.contig1.ptr(); s.contig2 = c.contig2.ptr(); s.bp1 = c.bp1.ptr(); s.bp2 = c.bp2.ptr();
-	s.dir1 = c.dir1.ptr(); s.dir2 = c.dir2.ptr(); s.bits = c.bits.ptr();
+	s.dir1 = c.dir1.ptr(); s.dir2 = c.dir2.ptr(); s.bits = c.bits.ptr(); s.bits2 = c.bits2.ptr();
 	s.split_reads1 = c.split_reads1.ptr(); s.split_reads2 = c.split_reads2.ptr(); s.discordant_mates = c.discordant_mates.ptr(); s.filter = c.filter.ptr(); s.evalue = c.evalue.ptr();
 	s.n_list1 = n1; s.n_list2 = n2;
 	return s;

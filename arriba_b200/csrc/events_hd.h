@@ -16,7 +16,7 @@ namespace arb {
 
 struct cand_state { // mutable event-level columns, device copies
 	u32 n;
-	const u32* gene1; const u32* gene2; const u16* contig1; const u16* contig2; const i32* bp1; const i32* bp2; const u8* dir1; const u8* dir2; const u8* bits;
+	const u32* gene1; const u32* gene2; const u16* contig1; const u16* contig2; const i32* bp1; const i32* bp2; const u8* dir1; const u8* dir2; const u8* bits; const u8* bits2; // bits2: 1 = transcript start ambiguous
 	u32* split_reads1; u32* split_reads2; u32* discordant_mates; u8* filter; float* evalue;
 	u32* n_list1; u32* n_list2; // current sizes of the split-read lists (grow when ITD lists are merged)
 };
@@ -25,6 +25,11 @@ ARB_HD bool cand_is_itd(const cand_state& c, u32 k, u32 max_itd_length) { // com
 	return c.gene1[k] == c.gene2[k] && ((u32) c.bp2[k] - (u32) c.bp1[k]) < max_itd_length && c.dir1[k] == UPSTREAM && c.dir2[k] == DOWNSTREAM;
 }
 ARB_HD u32 cand_support(const cand_state& c, u32 k) { return c.split_reads1[k] + c.split_reads2[k] + c.discordant_mates[k]; }
+ARB_HD bool cand_both_spliced(const cand_state& c, const annot_view& an, u32 k) { // both_breakpoints_spliced (common.hpp:280-284)
+	const u8 bits = c.bits[k];
+	const bool f1 = an.gene_strand[c.gene1[k]], f2 = an.gene_strand[c.gene2[k]];
+	return (bits & CB_SPLICED1) && (bits & CB_SPLICED2) && ((f1 == f2 && c.dir1[k] != c.dir2[k]) || (f1 != f2 && c.dir1[k] == c.dir2[k]));
+}
 
 struct merge_eligible_fn { // candidates that take part: unfiltered, or ITD-shaped (merge_adjacent_fusions.cpp:23-26)
 	cand_state c; u32 max_itd_length; u32* flag;
@@ -370,11 +375,7 @@ struct in_vitro_fn {
 struct spliced_support_fn {
 	cand_state c; frag_view f; annot_view an; coverage_view cov; const u32* reads_by_gene; u32 threshold;
 	const u32* l1o; const u32* l1; const u32* l2o; const u32* l2; const u32* ldo; const u32* ld; u32* support; // 0xFFFFFFFF: not eligible
-	ARB_HD bool both_spliced(u32 k) const { // common.hpp:280-284
-		const u8 bits = c.bits[k];
-		const bool f1 = an.gene_strand[c.gene1[k]], f2 = an.gene_strand[c.gene2[k]];
-		return (bits & CB_SPLICED1) && (bits & CB_SPLICED2) && ((f1 == f2 && c.dir1[k] != c.dir2[k]) || (f1 != f2 && c.dir1[k] == c.dir2[k]));
-	}
+	ARB_HD bool both_spliced(u32 k) const { return cand_both_spliced(c, an, k); }
 	ARB_HD bool long_exon_at(u16 contig, i32 bp) const { // any exon over the breakpoint longer than 1000 bases (a point query returns the region's items)
 		if (contig >= an.n_contigs) return false;
 		const u32 lo = an.exon_region_begin[contig], hi = an.exon_region_begin[contig + 1];

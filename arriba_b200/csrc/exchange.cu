@@ -156,7 +156,7 @@ void engine::exchange_commit(int group) {
 			frags.swapped.zero(ex, frags.n);
 			push_open = true; // finish_push closes it
 			finish_push(n_gene_entries);
-			filters_done = false; cands.n = 0; cands.genomic_marked = false;
+			filters_done = false; cands.n = 0; cands.genomic_marked = false; has_tag_csr = false;
 			ex.sync();
 			break;
 		case XG_MISMAP_STATE: ex.sync(); break;
@@ -276,7 +276,7 @@ void engine::candidates_import(const void* all_blobs, u64 stride, const u64* siz
 	copy_dd(ex, key.ptr(), src.first_frag.ptr(), (u64) C * 4);
 	iota_fn io = {perm.ptr()}; for_each(ex, C, io);
 	radix_sort_pairs_u32(ex, key.ptr(), perm.ptr(), tk.ptr(), tv.ptr(), C, bits_for_u32(frags.n + 1));
-	cands.n = C; cands.genomic_marked = false;
+	cands.n = C; cands.genomic_marked = false; has_tag_csr = false;
 	cands.gene1.ensure(C); cands.gene2.ensure(C); cands.contig1.ensure(C); cands.contig2.ensure(C); cands.bp1.ensure(C); cands.bp2.ensure(C); cands.dir1.ensure(C); cands.dir2.ensure(C);
 	cands.split_reads1.ensure(C); cands.split_reads2.ensure(C); cands.discordant_mates.ensure(C); cands.filter.ensure(C); cands.bits.ensure(C); cands.bits2.ensure(C);
 	cands.anchor1.ensure(C); cands.anchor2.ensure(C); cands.evalue.ensure(C); cands.first_frag.ensure(C);

@@ -163,7 +163,7 @@ void engine::find_fusions(i32 max_mate_gap) {
 	for_each(ex, C, ff);
 
 	// 4. pass A
-	cands.n = C; cands.genomic_marked = false;
+	cands.n = C; cands.genomic_marked = false; has_tag_csr = false;
 	cands.gene1.ensure(C); cands.gene2.ensure(C); cands.contig1.ensure(C); cands.contig2.ensure(C); cands.bp1.ensure(C); cands.bp2.ensure(C);
 	cands.dir1.ensure(C); cands.dir2.ensure(C); cands.split_reads1.ensure(C); cands.split_reads2.ensure(C); cands.discordant_mates.ensure(C);
 	cands.filter.ensure(C); cands.bits.ensure(C); cands.bits2.ensure(C); cands.anchor1.ensure(C); cands.anchor2.ensure(C); cands.evalue.ensure(C);

@@ -1,6 +1,9 @@
 // blacklist.cpp -- the rules of a blacklist file (-b), read like filter_blacklisted_ranges does (filter_blacklisted_ranges.cpp:17-120, :252-268): two columns
 // per line, each a gene name, a position or a range (contig:start-end, optionally with a strand prefix and a trailing '*' on the contig), or in column 2 a keyword.
-// The rules go to the device in file order (arb_set_blacklist), which matches them to the candidates (csrc/blacklist_hd.h).
+// Files of known fusions (-k, recover_known_fusions.cpp:21-38) and tags (-t, annotate_tags.cpp:11-43) have the same two columns without keywords; a tags
+// file has a third column, the tag.
+// The rules go to the device in file order (arb_set_blacklist / arb_set_known_fusions / arb_set_tags), which matches them to the candidates (csrc/blacklist_hd.h).
+#include <algorithm>
 #include <climits>
 #include <iostream>
 #include <stdexcept>
@@ -14,10 +17,10 @@ namespace {
 struct rule_item { u8 type, strand; u16 contig; i32 start, end; u32 gene; };
 
 struct rule_reader {
-	const refdata& ref; const std::string& path; size_t line_no; const std::string* line;
+	const refdata& ref; const std::string& path; const char* kind; size_t line_no; const std::string* line;
 
 	[[noreturn]] void undefined(const std::string& why) const {
-		throw std::runtime_error("blacklist '" + path + "', line " + std::to_string((unsigned long long) line_no) + ": " + why + ": " + *line);
+		throw std::runtime_error(std::string(kind) + " '" + path + "', line " + std::to_string((unsigned long long) line_no) + ": " + why + ": " + *line);
 	}
 
 	// parse_range (:17-80); every failure but an unmatched wildcard prints the same warning, with the text as the reference holds it by then (last ':' a tab)
@@ -76,34 +79,58 @@ struct rule_reader {
 		return true;
 	}
 
-	// the bins of a positional item (:272-275) must be computable in int: start - max_mate_gap and end + max_mate_gap + 99999 (get_genome_bins_from_range)
-	void check_bins(const rule_item& item, i32 max_mate_gap) const {
+	// the bins of a positional item (:272-275) must be computable in int: start - widen and end + widen + 99999 (get_genome_bins_from_range)
+	void check_bins(const rule_item& item, i32 widen) const {
 		if (item.type != ARB_RULE_POSITION && item.type != ARB_RULE_RANGE && item.type != ARB_RULE_GENE) return;
-		if ((i64) item.start - max_mate_gap < INT_MIN || (i64) item.end + max_mate_gap + 99999 > INT_MAX)
-			undefined("the coordinates widened by the maximum mate gap (" + std::to_string(max_mate_gap) + ") overflow int");
+		if ((i64) item.start - widen < INT_MIN || (i64) item.end + widen + 99999 > INT_MAX) {
+			if (widen) undefined("the coordinates widened by the maximum mate gap (" + std::to_string(widen) + ") overflow int");
+			undefined("the coordinates overflow int");
+		}
 	}
 };
 
 } // namespace
 
-void read_fusion_rules(const std::string& path, const refdata& ref, i32 max_mate_gap, fusion_rules& out) {
+// kind BLACKLIST: keywords in column 2, bins widened by max_mate_gap (filter_blacklisted_ranges.cpp:252-275); KNOWN_FUSIONS: no keywords, bins not widened
+// (recover_known_fusions.cpp:23-37); TAGS: the same plus the third column, checked before the items and sanitised (annotate_tags.cpp:14-33)
+void read_fusion_rules(const std::string& path, const refdata& ref, rule_file kind, i32 max_mate_gap, fusion_rules& out) {
+	static const char* KIND[] = {"blacklist", "known fusions", "tags"};
 	std::string text;
 	read_whole_file(path, text);
 	out = fusion_rules();
-	rule_reader r = {ref, path, 0, NULL};
+	rule_reader r = {ref, path, KIND[kind], 0, NULL};
+	const i32 widen = kind == RULES_BLACKLIST ? max_mate_gap : 0;
 	size_t at = 0; std::string line;
 	while (next_line(text, at, line)) {
 		++r.line_no; r.line = &line;
 		if (line.empty() || line[0] == '#') continue;
 		tsv_fields f(line);
 		const std::string range1 = f.next(), range2 = f.next(); // further columns are ignored
+		std::string tag;
+		if (kind == RULES_TAGS) {
+			tag = f.next();
+			if (tag.empty()) { std::cerr << "WARNING: encountered a line with an empty tag => skipped" << std::endl; continue; }
+		}
 		rule_item a, b;
-		if (!r.parse_item(range1, a, false) || !r.parse_item(range2, b, true)) continue; // column 2 is parsed only if column 1 was
-		r.check_bins(a, max_mate_gap); r.check_bins(b, max_mate_gap);
+		if (!r.parse_item(range1, a, false) || !r.parse_item(range2, b, kind == RULES_BLACKLIST)) continue; // column 2 is parsed only if column 1 was
+		r.check_bins(a, widen); r.check_bins(b, widen);
 		out.type1.push_back(a.type); out.type2.push_back(b.type); out.strand1.push_back(a.strand); out.strand2.push_back(b.strand);
 		out.contig1.push_back(a.contig); out.contig2.push_back(b.contig); out.start1.push_back(a.start); out.end1.push_back(a.end);
 		out.start2.push_back(b.start); out.end2.push_back(b.end); out.gene1.push_back(a.gene); out.gene2.push_back(b.gene);
+		if (kind == RULES_TAGS) {
+			for (size_t x = 0; x < tag.size(); ++x) if ((signed char) tag[x] < '!' || (signed char) tag[x] > '~' || tag[x] == ',') tag[x] = '_'; // char is signed: bytes >= 0x80 too
+			out.tag.push_back(tag);
+		}
 	}
+}
+
+// the distinct tags in bytewise order (std::set<std::string>, annotate_tags.cpp:55) and the rank of every rule's tag among them
+void rank_tags(const fusion_rules& r, std::vector<std::string>& distinct, std::vector<u32>& rank) {
+	distinct = r.tag;
+	std::sort(distinct.begin(), distinct.end());
+	distinct.erase(std::unique(distinct.begin(), distinct.end()), distinct.end());
+	rank.resize(r.tag.size());
+	for (size_t k = 0; k < r.tag.size(); ++k) rank[k] = (u32) (std::lower_bound(distinct.begin(), distinct.end(), r.tag[k]) - distinct.begin());
 }
 
 }} // namespace

@@ -770,7 +770,7 @@ void pipeline::filter_blacklist() {
 	std::vector<u32> ids;
 	for (u32 k = 0; k < ev.n; ++k) if (ev.filter[k] == F_none || ev.genomic_support(k)) ids.push_back(k); // :238-239
 	fusion_rules r;
-	read_fusion_rules(opt.blacklist_file, ref, max_mate_gap, r);
+	read_fusion_rules(opt.blacklist_file, ref, RULES_BLACKLIST, max_mate_gap, r);
 	const uint32_t n = (uint32_t) r.size();
 	check(ctx, arb_set_blacklist(ctx, n, r.type1.data(), r.type2.data(), r.strand1.data(), r.strand2.data(), r.contig1.data(), r.contig2.data(),
 	                             r.start1.data(), r.end1.data(), r.start2.data(), r.end2.data(), r.gene1.data(), r.gene2.data()), "arb_set_blacklist");
@@ -779,6 +779,63 @@ void pipeline::filter_blacklist() {
 	check(ctx, arb_filter_blacklist(ctx, (uint32_t) ids.size(), ids.data(), opt.params.evalue_cutoff, max_mate_gap, verdict.data(), &blacklisted), "arb_filter_blacklist");
 	for (size_t x = 0; x < ids.size(); ++x) if (verdict[x]) ev.filter[ids[x]] = F_blacklist; // overwrites an earlier filter of a candidate with genomic support
 	log_remaining(("Filtering blacklisted fusions in '" + opt.blacklist_file + "'").c_str());
+}
+
+// ------------------------------------------------------------------------------------------- known fusions (-k)
+// recover_known_fusions.cpp:14-100, right after filter_both_intronic: candidates that min_support or relative_support removed come back if a rule of the file
+// matches them (csrc/blacklist_hd.h). The device reads the support counts, the spliced bits and the coverage windows, so the host's state goes up first.
+void pipeline::recover_known_fusions() {
+	fusion_rules r;
+	read_fusion_rules(opt.known_fusions_file, ref, RULES_KNOWN_FUSIONS, max_mate_gap, r);
+	std::vector<u32> ids;
+	for (u32 k = 0; k < ev.n; ++k)
+		if ((ev.filter[k] == F_relative_support || ev.filter[k] == F_min_support) && ev.gene1[k] != ev.gene2[k]) ids.push_back(k); // :43-50
+	const uint32_t n = (uint32_t) r.size();
+	check(ctx, arb_set_known_fusions(ctx, n, r.type1.data(), r.type2.data(), r.strand1.data(), r.strand2.data(), r.contig1.data(), r.contig2.data(),
+	                                 r.start1.data(), r.end1.data(), r.start2.data(), r.end2.data(), r.gene1.data(), r.gene2.data()), "arb_set_known_fusions");
+	if (!ids.empty()) {
+		ensure_coverage_on_device();
+		push_candidate_state();
+		std::vector<u8> verdict(ids.size());
+		uint32_t rescued = 0;
+		check(ctx, arb_recover_known_fusions(ctx, (uint32_t) ids.size(), ids.data(), max_mate_gap, verdict.data(), &rescued), "arb_recover_known_fusions");
+		for (size_t x = 0; x < ids.size(); ++x) if (verdict[x]) ev.filter[ids[x]] = F_none;
+	}
+	log_remaining(("Searching for known fusions in '" + opt.known_fusions_file + "'").c_str());
+}
+
+// ------------------------------------------------------------------------------------------- tags (-t)
+// load_tags (annotate_tags.cpp:11-43) and annotate_tags (:45-83) for every row that is written: the rows of fusions.tsv and, with a discarded file, all others.
+// The device keeps the tags of every candidate for the rows it formats; the host keeps a copy for the rows it formats itself.
+void pipeline::annotate_tags() {
+	say("Loading tags from '" + opt.tags_file + "'");
+	fusion_rules r;
+	read_fusion_rules(opt.tags_file, ref, RULES_TAGS, max_mate_gap, r);
+	std::vector<u32> rank;
+	rank_tags(r, tag_names, rank);
+	std::vector<char> chars; std::vector<u32> off(1, 0);
+	for (size_t t = 0; t < tag_names.size(); ++t) { chars.insert(chars.end(), tag_names[t].begin(), tag_names[t].end()); off.push_back((u32) chars.size()); }
+	chars.push_back(0); rank.push_back(0);
+	const uint32_t n = (uint32_t) r.size();
+	check(ctx, arb_set_tags(ctx, n, r.type1.data(), r.type2.data(), r.strand1.data(), r.strand2.data(), r.contig1.data(), r.contig2.data(), r.start1.data(), r.end1.data(),
+	                        r.start2.data(), r.end2.data(), r.gene1.data(), r.gene2.data(), rank.data(), (uint32_t) tag_names.size(), chars.data(), off.data()), "arb_set_tags");
+	const bool all = !opt.discarded_output_file.empty();
+	std::vector<u32> ids;
+	for (u32 k = 0; k < ev.n; ++k) if (all || ev.filter[k] == F_none) ids.push_back(k);
+	push_candidate_state();
+	uint64_t pairs = 0;
+	if (arb_annotate_tags(ctx, (uint32_t) ids.size(), ids.data(), max_mate_gap, &pairs) != 0) throw std::runtime_error("tags '" + opt.tags_file + "': " + arb_last_error(ctx));
+	tag_off.assign((size_t) ev.n + 1, 0); tag_ranks.assign(pairs ? pairs : 1, 0);
+	check(ctx, arb_get_tags(ctx, tag_off.data(), tag_ranks.data()), "arb_get_tags");
+	tags_loaded = true;
+}
+
+// the tags column of candidate k (annotate_tags.cpp:72-82)
+std::string pipeline::tags_of(u32 k) const {
+	if (!tags_loaded || tag_off[k] == tag_off[k + 1]) return ".";
+	std::string out;
+	for (u32 x = tag_off[k]; x < tag_off[k + 1]; ++x) { if (x > tag_off[k]) out += ','; out += tag_names[tag_ranks[x]]; }
+	return out;
 }
 
 void pipeline::assign_confidence() { // filter_genomic_support.cpp:222-402

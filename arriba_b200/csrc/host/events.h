@@ -47,11 +47,14 @@ void read_genomic_breakpoints(const std::string& path, const std::map<std::strin
 
 // rules of a blacklist file (blacklist.cpp), in file order: the two items of every line that parse_blacklist_item accepted, one column per field (type: ARB_RULE_*,
 // strand: ARB_RULE_STRAND_*, coordinates 0-based; gene: the gene of a GENE item). Lines it rejects print the reference's WARNING on stderr. A file of known
-// fusions (-k) has the same format.
+// fusions (-k) and a tags file (-t) have the same format; a tags file adds the tag of every rule, sanitised.
 struct fusion_rules {
 	std::vector<u8> type1, type2, strand1, strand2; std::vector<u16> contig1, contig2; std::vector<i32> start1, end1, start2, end2; std::vector<u32> gene1, gene2;
+	std::vector<std::string> tag;
 	size_t size() const { return type1.size(); }
 };
-void read_fusion_rules(const std::string& path, const refdata& ref, i32 max_mate_gap, fusion_rules& out);
+enum rule_file { RULES_BLACKLIST = 0, RULES_KNOWN_FUSIONS = 1, RULES_TAGS = 2 };
+void read_fusion_rules(const std::string& path, const refdata& ref, rule_file kind, i32 max_mate_gap, fusion_rules& out);
+void rank_tags(const fusion_rules& r, std::vector<std::string>& distinct, std::vector<u32>& rank);
 
 }} // namespace

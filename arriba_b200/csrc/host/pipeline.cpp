@@ -171,7 +171,10 @@ void pipeline::events_until(int last) { // arriba.cpp:420-545, filters enabled b
 			case EV_MIN_SUPPORT: if (on(F_min_support)) filter_min_support(); break;
 			case EV_RELATIVE_SUPPORT: if (on(F_relative_support)) filter_relative_support(); break;
 			case EV_ITD: if (on(F_internal_tandem_duplication)) recover_internal_tandem_duplication(); break;
-			case EV_INTRONIC: if (on(F_intronic)) filter_both_intronic(); break;
+			case EV_INTRONIC: // arriba.cpp:469-478: the known fusions follow the intronic filter in the same stage
+				if (on(F_intronic)) filter_both_intronic();
+				if (on(F_known_fusions) && !opt.known_fusions_file.empty()) recover_known_fusions();
+				break;
 			case EV_IN_VITRO: if (on(F_in_vitro)) filter_in_vitro(); break;
 			case EV_SPLICED: if (on(F_spliced)) recover_both_spliced(); break;
 			case EV_SELECT_BEST: if (on(F_select_best)) select_best(); break;

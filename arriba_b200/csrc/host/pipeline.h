@@ -36,6 +36,7 @@ struct run_options { // options_t (options.hpp:25-69) restricted to what this im
 	unsigned top_viral_contigs; float viral_contig_min_covered_fraction; // -T 5, -C 0.05
 	std::string genomic_breakpoints_file; unsigned max_genomic_breakpoint_distance; // -d (empty: none), -D 100000
 	std::string blacklist_file; // -b (empty: none)
+	std::string known_fusions_file, tags_file; // -k, -t (empty: none)
 	run_options();
 };
 
@@ -71,6 +72,9 @@ struct pipeline {
 	void recover_many_spliced(); void filter_short_anchor(); void filter_end_to_end(); void filter_no_coverage(); void recover_isoforms(); void assign_confidence();
 	void mark_genomic_support(); void filter_no_genomic_support(); void recover_genomic_support(); // -d (filter_genomic_support.cpp)
 	void filter_blacklist(); // -b (filter_blacklisted_ranges.cpp)
+	void recover_known_fusions(); // -k (recover_known_fusions.cpp)
+	void annotate_tags(); std::string tags_of(u32 k) const; // -t (annotate_tags.cpp): the tags of every written row, ranks per candidate
+	std::vector<std::string> tag_names; std::vector<u32> tag_off, tag_ranks; bool tags_loaded = false;
 	void write_output();
 	void make_kmer_index(); void filter_homologs(); void filter_mismappers(); bool splice_sites_ready;
 	void find_top_expressed_genes(std::vector<u32>& reads_by_gene, std::vector<u8>& present, unsigned int& threshold, float quantile);

@@ -48,6 +48,9 @@ void engine::format_discarded_rows(const u8* confidence, u64* n_rows, u64* n_byt
 	fm.t.exon_prev = row_exon_prev.ptr(); fm.t.exon_next = row_exon_next.ptr(); fm.t.confidence = conf.ptr();
 	fm.t.closest1 = cands.genomic_marked ? cands.closest1.ptr() : NULL; fm.t.closest2 = cands.genomic_marked ? cands.closest2.ptr() : NULL;
 	fm.t.cov.windows = coverage_windows.ptr(); fm.t.cov.contig_off = coverage_off.ptr(); fm.t.cov.contig_windows = coverage_n.ptr(); fm.t.cov.n_contigs = coverage_contigs;
+	const bool tags = has_tag_csr && tag_csr_n == C; // arb_annotate_tags ran on this candidate table
+	fm.t.tag_text.chars = tags ? tag_text.ptr() : NULL; fm.t.tag_text.off = tags ? tag_text_off.ptr() : NULL;
+	fm.t.tag_off = tags ? tag_csr_off.ptr() : NULL; fm.t.tag_rank = tags ? tag_csr_rank.ptr() : NULL;
 	for (int k = 0; k < ARB_N_FILTERS; ++k) fm.t.filters_by_name[k] = row_filters_by_name[k];
 	fm.t.max_itd_length = row_max_itd_length;
 	fm.l1o = cands.list1_off.ptr(); fm.l1 = cands.list1.ptr(); fm.l2o = cands.list2_off.ptr(); fm.l2 = cands.list2.ptr(); fm.ldo = cands.listd_off.ptr(); fm.ld = cands.listd.ptr();

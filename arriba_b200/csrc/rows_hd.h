@@ -21,6 +21,7 @@ struct row_tables { // what the rows need besides the candidate state, the fragm
 	const u8* confidence;                          // per candidate
 	const i32* closest1; const i32* closest2;      // closest genomic breakpoints per candidate (-d), NULL: none marked
 	coverage_view cov;
+	text_pool tag_text; const u32* tag_off; const u32* tag_rank; // -t: distinct tags by rank, and the ranks of every candidate's tags (CSR); NULL: no tags
 	u8 filters_by_name[ARB_N_FILTERS];             // filter ids in alphabetical order of their names
 	u32 max_itd_length;
 };
@@ -144,6 +145,11 @@ struct row_formatter {
 		for (u32 p = off[k]; p < off[k + 1]; ++p) { const u8 l = f.filter[list[p]]; if (l != F_none && l < ARB_N_FILTERS) { present |= (u64) 1 << l; ++count[l]; } }
 	}
 
+	template <class W> ARB_HD void tags(W& w, u32 k) const { // annotate_tags.cpp:72-82: the distinct tags joined by ',', in bytewise order
+		if (!t.tag_off || t.tag_off[k] == t.tag_off[k + 1]) { w.put('.'); return; }
+		for (u32 x = t.tag_off[k]; x < t.tag_off[k + 1]; ++x) { if (x > t.tag_off[k]) w.put(','); put_pool(w, t.tag_text, t.tag_rank[x]); }
+	}
+
 	template <class W> ARB_HD void row(W& w, u32 k) const {
 		const u8 bits = c.bits[k];
 		u32 site5 = site(c.gene1[k], bits & CB_SPLICED1, bits & CB_EXONIC1, c.contig1[k], c.bp1[k]), site3 = site(c.gene2[k], bits & CB_SPLICED2, bits & CB_EXONIC2, c.contig2[k], c.bp2[k]);
@@ -162,7 +168,9 @@ struct row_formatter {
 		if (cov3 >= 0) put_int(w, cov3); else w.put('.');
 		w.put('\t');
 		switch (t.confidence[k] & 3) { case 0: put_text(w, "low"); break; case 1: put_text(w, "medium"); break; default: put_text(w, "high"); break; }
-		put_text(w, "\t.\t.\t.\t"); // reading frame, tags, retained protein domains
+		put_text(w, "\t.\t"); // reading frame
+		tags(w, k);
+		put_text(w, "\t.\t"); // retained protein domains
 		genomic_breakpoint(w, c5, b5, gb5); w.put('\t'); genomic_breakpoint(w, c3, b3, gb3);
 		u32 count[ARB_N_FILTERS]; u64 present = 0;
 		for (u32 x = 0; x < ARB_N_FILTERS; ++x) count[x] = 0;

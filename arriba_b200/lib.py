@@ -66,7 +66,8 @@ class Timings(C.Structure):
                 ("mismapper_items", C.c_uint64), ("kmer_positions", C.c_uint64), ("mismapper_heavy_items", C.c_uint64),
                 ("mismappers_pass1_ms", C.c_float), ("mismappers_pass2_ms", C.c_float), ("mismapper_tasks", C.c_uint64), ("mismapper_rounds", C.c_uint32), ("mismapper_overflow", C.c_uint32), ("mismapper_table_slots", C.c_uint32),
                 ("cascade_head_ms", C.c_float), ("cascade_sequences_ms", C.c_float), ("cascade_queued", C.c_uint64), ("cascade_algorithmic_bytes", C.c_uint64 * 2), ("annotate_ms", C.c_float), ("in_vitro_ms", C.c_float), ("multimappers_ms", C.c_float), ("order_ms", C.c_float), ("partners_ms", C.c_float), ("rows_ms", C.c_float), ("bam_scan_ms", C.c_float), ("consensus_ms", C.c_float), ("mismapper_algorithmic_bytes", C.c_uint64), ("mismapper_sequences", C.c_uint64), ("mismapper_hits", C.c_uint64),
-                ("genomic_support_ms", C.c_float), ("blacklist_ms", C.c_float)]
+                ("genomic_support_ms", C.c_float), ("blacklist_ms", C.c_float), ("known_fusions_ms", C.c_float), ("tags_ms", C.c_float),
+                ("tags_match_ms", C.c_float), ("tags_sort_ms", C.c_float), ("tags_pairs", C.c_uint64)]
 
 
 _CTYPE = {np.dtype(np.uint8): C.c_uint8, np.dtype(np.uint16): C.c_uint16, np.dtype(np.uint32): C.c_uint32, np.dtype(np.int32): C.c_int32,
@@ -131,6 +132,11 @@ def load(path=None):
                        ("arb_mark_genomic_support", [C.c_int32, C.c_int32, _p(C.c_uint32)]), ("arb_get_genomic_support", [_p(C.c_int32), _p(C.c_int32)]),
                        ("arb_set_blacklist", [C.c_uint32] + [_p(C.c_uint8)] * 4 + [_p(C.c_uint16)] * 2 + [_p(C.c_int32)] * 4 + [_p(C.c_uint32)] * 2),
                        ("arb_filter_blacklist", [C.c_uint32, _p(C.c_uint32), C.c_float, C.c_int32, _p(C.c_uint8), _p(C.c_uint32)]),
+                       ("arb_set_known_fusions", [C.c_uint32] + [_p(C.c_uint8)] * 4 + [_p(C.c_uint16)] * 2 + [_p(C.c_int32)] * 4 + [_p(C.c_uint32)] * 2),
+                       ("arb_recover_known_fusions", [C.c_uint32, _p(C.c_uint32), C.c_int32, _p(C.c_uint8), _p(C.c_uint32)]),
+                       ("arb_set_tags", [C.c_uint32] + [_p(C.c_uint8)] * 4 + [_p(C.c_uint16)] * 2 + [_p(C.c_int32)] * 4 + [_p(C.c_uint32)] * 2 + [_p(C.c_uint32), C.c_uint32, C.c_char_p, _p(C.c_uint32)]),
+                       ("arb_annotate_tags", [C.c_uint32, _p(C.c_uint32), C.c_int32, _p(C.c_uint64)]),
+                       ("arb_get_tags", [_p(C.c_uint32), _p(C.c_uint32)]),
                        ("arb_set_candidate_state", [_p(C.c_uint8), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_float)]),
                        ("arb_set_candidate_lists", [_p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32)]),
                        ("arb_set_splice_sites", [_p(C.c_uint32), _p(C.c_int32)]),
@@ -354,6 +360,49 @@ class Context:
         self._check(self.lib.arb_filter_blacklist(self.h, ids.size, ptr(ids if ids.size else np.zeros(1, np.uint32)), float(evalue_cutoff), int(max_mate_gap), ptr(out), C.byref(n)))
         return out[:ids.size]
 
+    # ---- known fusions (-k) and tags (-t): the same rule columns as set_blacklist
+    def _rule_columns(self, rules):
+        cols = [np.ascontiguousarray(rules[k], dt) for k, dt in self.RULE_COLUMNS]
+        n = cols[0].size
+        assert all(c.size == n for c in cols), "columns differ in length"
+        return n, [c if c.size else np.zeros(1, c.dtype) for c in cols]
+
+    def set_known_fusions(self, rules):
+        n, cols = self._rule_columns(rules)
+        self._check(self.lib.arb_set_known_fusions(self.h, n, *[ptr(c) for c in cols]))
+
+    def recover_known_fusions(self, ids, max_mate_gap=0):
+        """Verdicts (1 = rescued) of the candidates `ids` (filter relative_support or min_support, gene1 != gene2) against the rules of set_known_fusions."""
+        ids = np.ascontiguousarray(ids, np.uint32)
+        out = np.zeros(max(ids.size, 1), np.uint8); n = C.c_uint32()
+        self._check(self.lib.arb_recover_known_fusions(self.h, ids.size, ptr(ids if ids.size else np.zeros(1, np.uint32)), int(max_mate_gap), ptr(out), C.byref(n)))
+        return out[:ids.size]
+
+    def set_tags(self, rules, tags):
+        """rules: as set_blacklist; tags: the (sanitised) tag of every rule, bytes or str."""
+        n, cols = self._rule_columns(rules)
+        tags = [t.encode("latin-1") if isinstance(t, str) else bytes(t) for t in tags]
+        assert len(tags) == n, "one tag per rule"
+        distinct = sorted(set(tags))
+        rank = np.array([distinct.index(t) for t in tags] if n else [0], np.uint32)
+        off = np.zeros(len(distinct) + 1, np.uint32); off[1:] = np.cumsum([len(t) for t in distinct]) if distinct else []
+        chars = b"".join(distinct) + b"\0"
+        self._keep.append(chars)
+        self._check(self.lib.arb_set_tags(self.h, n, *[ptr(c) for c in cols], ptr(rank), len(distinct), chars, ptr(off)))
+        self._tag_names = distinct
+
+    def annotate_tags(self, ids, max_mate_gap=0):
+        """The tags of the rows `ids`: a list per candidate (all candidates; the ones not in `ids` have none), each sorted bytewise, as bytes."""
+        ids = np.ascontiguousarray(ids, np.uint32)
+        pairs = C.c_uint64()
+        self._check(self.lib.arb_annotate_tags(self.h, ids.size, ptr(ids if ids.size else np.zeros(1, np.uint32)), int(max_mate_gap), C.byref(pairs)))
+        n = C.c_uint32(); n1 = C.c_uint64(); n2 = C.c_uint64(); nd = C.c_uint64()
+        self._check(self.lib.arb_candidates_size(self.h, C.byref(n), C.byref(n1), C.byref(n2), C.byref(nd)))
+        n = n.value
+        off = np.zeros(n + 1, np.uint32); ranks = np.zeros(max(int(pairs.value), 1), np.uint32)
+        self._check(self.lib.arb_get_tags(self.h, ptr(off), ptr(ranks)))
+        return [[self._tag_names[r] for r in ranks[off[k]:off[k + 1]]] for k in range(n)]
+
     def slot_swaps(self):
         s = np.zeros(self.n_fragments, np.uint8)
         self._check(self.lib.arb_get_slot_swaps(self.h, ptr(s)))
@@ -416,7 +465,8 @@ class RunOptions(C.Structure):
                 ("exonic_fraction", C.c_float), ("min_itd_allele_fraction", C.c_float), ("min_itd_support", C.c_uint32),
                 ("print_extra_info_for_discarded_fusions", C.c_int32), ("echo_progress", C.c_int32),
                 ("top_viral_contigs", C.c_uint32), ("viral_contig_min_covered_fraction", C.c_float),
-                ("genomic_breakpoints_file", C.c_char_p), ("max_genomic_breakpoint_distance", C.c_uint32), ("blacklist_file", C.c_char_p)]
+                ("genomic_breakpoints_file", C.c_char_p), ("max_genomic_breakpoint_distance", C.c_uint32), ("blacklist_file", C.c_char_p),
+                ("known_fusions_file", C.c_char_p), ("tags_file", C.c_char_p)]
 
 
 class RunStats(C.Structure):
@@ -462,7 +512,7 @@ class Pipeline:
     """One run of the hot path on files: the call a user of the library makes (the `arriba` CLI is a thin wrapper over it)."""
 
     def __init__(self, bam, gtf, fasta, threads=1, device=0, lib_path=None, strandedness=3, params=None, output=None, discarded=None,
-                 genomic_breakpoints=None, max_genomic_breakpoint_distance=100000, blacklist=None):
+                 genomic_breakpoints=None, max_genomic_breakpoint_distance=100000, blacklist=None, known_fusions=None, tags=None):
         self.lib = load(lib_path)
         _load_pipeline_api(self.lib)
         o = RunOptions()
@@ -478,6 +528,10 @@ class Pipeline:
         o.max_genomic_breakpoint_distance = max_genomic_breakpoint_distance
         if blacklist:  # read only while the blacklist filter is on (params.filter_mask bit 20)
             self._strings.append(blacklist.encode()); o.blacklist_file = self._strings[-1]
+        if known_fusions:  # read only while the known_fusions filter is on (params.filter_mask bit 18)
+            self._strings.append(known_fusions.encode()); o.known_fusions_file = self._strings[-1]
+        if tags:
+            self._strings.append(tags.encode()); o.tags_file = self._strings[-1]
         o.threads = threads; o.device = device; o.strandedness = strandedness
         if params is not None:
             o.params = params

@@ -350,6 +350,29 @@ int arb_set_blacklist(arb_ctx* ctx, uint32_t n, const uint8_t* type1, const uint
                       const uint32_t* gene1, const uint32_t* gene2);
 int arb_filter_blacklist(arb_ctx* ctx, uint32_t n_ids, const uint32_t* ids, float evalue_cutoff, int32_t max_mate_gap, uint8_t* verdicts, uint32_t* n_blacklisted);
 
+/* ---- known fusions (-k) and tags (-t) ----------------------------------------------------------------------------------------------------------------------
+ * Both files have the blacklist's format and are passed as the same rule columns. Neither has keywords (parse_blacklist_item with allow_keyword = false), and
+ * the rules' bins are not widened by max_mate_gap.
+ * arb_set_known_fusions replaces the file loop of recover_known_fusions (source/recover_known_fusions.cpp:21-38). arb_recover_known_fusions replaces its
+ * search (:41-92) over the resident candidate table: one verdict byte per id in `ids` (the caller's eligible candidates: filter relative_support or
+ * min_support, gene1 != gene2), 1 = rescued; *n_rescued counts them. A rule matches directionally (item 1 the 5' gene, item 2 the 3' gene; also swapped when
+ * the transcript start is ambiguous and the breakpoints are not within 1 Mb on one contig). It rescues if both items are positions, the candidate has >= 2
+ * reads, or both breakpoints are spliced, the coverage of arb_set_coverage at them is < 200 and they are > 1 Mb apart or on different contigs.
+ * arb_set_tags replaces load_tags (source/annotate_tags.cpp:11-43): the rules, then tag_rank[rule] (< n_tags), the rank of the rule's sanitised tag among the
+ * distinct tags in bytewise order, and the texts of the n_tags distinct tags in that order (tag k = tag_chars[tag_off[k] .. tag_off[k + 1])).
+ * arb_annotate_tags replaces annotate_tags (:45-83) for the candidates `ids` (the rows that are written): the distinct tags of every row, ascending, stay on
+ * the device for arb_format_discarded_rows and come back with arb_get_tags: off[C + 1] over all C candidates (rows not in `ids` have none) and the
+ * *n_pairs ranks. It stops with an error when the rows and the rules make 2^31 or more (row, matching rule) pairs. */
+int arb_set_known_fusions(arb_ctx* ctx, uint32_t n, const uint8_t* type1, const uint8_t* type2, const uint8_t* strand1, const uint8_t* strand2,
+                          const uint16_t* contig1, const uint16_t* contig2, const int32_t* start1, const int32_t* end1, const int32_t* start2, const int32_t* end2,
+                          const uint32_t* gene1, const uint32_t* gene2);
+int arb_recover_known_fusions(arb_ctx* ctx, uint32_t n_ids, const uint32_t* ids, int32_t max_mate_gap, uint8_t* verdicts, uint32_t* n_rescued);
+int arb_set_tags(arb_ctx* ctx, uint32_t n, const uint8_t* type1, const uint8_t* type2, const uint8_t* strand1, const uint8_t* strand2,
+                 const uint16_t* contig1, const uint16_t* contig2, const int32_t* start1, const int32_t* end1, const int32_t* start2, const int32_t* end2,
+                 const uint32_t* gene1, const uint32_t* gene2, const uint32_t* tag_rank, uint32_t n_tags, const char* tag_chars, const uint32_t* tag_off);
+int arb_annotate_tags(arb_ctx* ctx, uint32_t n_ids, const uint32_t* ids, int32_t max_mate_gap, uint64_t* n_pairs);
+int arb_get_tags(arb_ctx* ctx, uint32_t* off, uint32_t* ranks);
+
 /* ---- device timing (CUDA events recorded on the context's stream around each stage) ---------------------------------- */
 typedef struct arb_timings {
 	float duplicates_ms;        /* duplicate marking (key build + hash group-by + mark) */
@@ -380,6 +403,11 @@ typedef struct arb_timings {
 	uint64_t mismapper_sequences, mismapper_hits; /* sequences searched by pass 1 (segment x gene x strand) and k-mer hits they visited */
 	float genomic_support_ms;   /* arb_mark_genomic_support: search of the sorted genomic breakpoints and the copy of the marks */
 	float blacklist_ms;         /* arb_filter_blacklist: key table of the rules, the search and the copy of the verdicts */
+	float known_fusions_ms;     /* arb_recover_known_fusions: key table of the rules, the search and the copy of the verdicts */
+	float tags_ms;              /* arb_annotate_tags: key table of the rules, both passes over the rows, the sort and the per-candidate table */
+	float tags_match_ms;        /* arb_annotate_tags, its first part: key table of the rules and both passes over the rows */
+	float tags_sort_ms;         /* arb_annotate_tags, its second part: sort of the (row, tag) pairs, duplicates removed, the per-candidate table */
+	uint64_t tags_pairs;        /* arb_annotate_tags: (row, matching rule) pairs before duplicates are removed (a rule counts once per bin it is met in) */
 } arb_timings;
 int arb_get_timings(arb_ctx* ctx, arb_timings* out);
 /* Device scratch memory is pooled per device and survives arb_ctx_destroy so that the next sample reuses it; this returns it to the driver
@@ -421,6 +449,8 @@ typedef struct arb_run_options {
 	const char* genomic_breakpoints_file;    /* -d: structural variants from whole-genome sequencing (four-column or VCF, optionally .gz), NULL = none */
 	uint32_t max_genomic_breakpoint_distance; /* -D 100000 */
 	const char* blacklist_file;      /* -b: blacklist rules (optionally .gz), NULL = none; read only while the blacklist filter is on */
+	const char* known_fusions_file;  /* -k: known fusions (optionally .gz), NULL = none; read only while the known_fusions filter is on */
+	const char* tags_file;           /* -t: tags (optionally .gz), NULL = none */
 } arb_run_options;
 void arb_default_run_options(arb_run_options* o);
 
