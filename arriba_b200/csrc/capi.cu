@@ -209,6 +209,14 @@ int arb_annotate_tags(arb_ctx* ctx, uint32_t n_ids, const uint32_t* ids, int32_t
 	ARB_API_BEGIN(ctx) const uint64_t p = ctx->e.annotate_tags(n_ids, ids, max_mate_gap); if (n_pairs) *n_pairs = p; ARB_API_END(ctx)
 }
 int arb_get_tags(arb_ctx* ctx, uint32_t* off, uint32_t* ranks) { ARB_API_BEGIN(ctx) ctx->e.get_tags(off, ranks); ARB_API_END(ctx) }
+int arb_set_protein_domains(arb_ctx* ctx, uint32_t n, const uint16_t* contig, const int32_t* start, const int32_t* end, const uint32_t* gene, const uint32_t* name_rank,
+                            uint32_t n_names, const char* name_chars, const uint32_t* name_off) {
+	ARB_API_BEGIN(ctx) ctx->e.set_protein_domains(n, contig, start, end, gene, name_rank, n_names, name_chars, name_off); ARB_API_END(ctx)
+}
+int arb_retained_protein_domains(arb_ctx* ctx, uint32_t n_ids, const uint32_t* ids, uint64_t* n_bytes) {
+	ARB_API_BEGIN(ctx) const uint64_t b = ctx->e.retained_protein_domains(n_ids, ids); if (n_bytes) *n_bytes = b; ARB_API_END(ctx)
+}
+int arb_get_retained_protein_domains(arb_ctx* ctx, uint64_t* off, char* text) { ARB_API_BEGIN(ctx) ctx->e.get_retained_protein_domains(off, text); ARB_API_END(ctx) }
 int arb_get_slot_swaps(arb_ctx* ctx, uint8_t* out) { ARB_API_BEGIN(ctx) ctx->e.get_slot_swaps(out); ARB_API_END(ctx) }
 
 } // extern "C"

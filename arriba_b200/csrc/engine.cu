@@ -14,7 +14,7 @@ void default_params(arb_params& p) { // options.cpp:71-107
 	p.max_mismapper_fraction = 0.8f; p.max_homolog_identity = 0.3f;
 }
 
-engine::engine(): row_max_itd_length(0), has_row_texts(false), row_text_bytes(0), kmer_block_shift(0), kmer_blocks(0), coverage_contigs(0), work_part(0), work_parts(1), mismap_items_total(0), mismap_ms_part(0), n_splice_sites(0), annot_pool_cap(0), n_dummy(0), n_gene_entries(0), push_cigar_ops(0), pool_workers(0), frag_name_bytes(0), rec_n(0), rec_arena_used(0), rec_carry(0), rec_carry_at(0), rec_expected_bytes(0), rec_cov_windows(0), rec_hash_mask(~(u64) 0), rec_n_tid(0), rec_n_contigs(0), rec_max_itd(0), rec_external_dup(false), rec_open(false), cascade_smem_bytes(0), cascade_resident_blocks(0), device(0), table_n(0), table_k(0), has_contigs(false), has_annotation(false), filters_done(false), merge_log_n(0), kmer_index_contigs(0), kmer_indexed(0), has_splice_sites(false), genomic_n(0), genomic_keys(0), genomic_heavy(0), has_genomic_breakpoints(false), n_tags(0), tag_csr_n(0), tag_csr_pairs(0), has_tags(false), has_tag_csr(false), blacklist_heavy(0), known_heavy(0), tags_heavy(0) {
+engine::engine(): row_max_itd_length(0), has_row_texts(false), row_text_bytes(0), kmer_block_shift(0), kmer_blocks(0), coverage_contigs(0), work_part(0), work_parts(1), mismap_items_total(0), mismap_ms_part(0), n_splice_sites(0), annot_pool_cap(0), n_dummy(0), n_gene_entries(0), push_cigar_ops(0), pool_workers(0), frag_name_bytes(0), rec_n(0), rec_arena_used(0), rec_carry(0), rec_carry_at(0), rec_expected_bytes(0), rec_cov_windows(0), rec_hash_mask(~(u64) 0), rec_n_tid(0), rec_n_contigs(0), rec_max_itd(0), rec_external_dup(false), rec_open(false), cascade_smem_bytes(0), cascade_resident_blocks(0), device(0), table_n(0), table_k(0), has_contigs(false), has_annotation(false), filters_done(false), merge_log_n(0), kmer_index_contigs(0), kmer_indexed(0), has_splice_sites(false), genomic_n(0), genomic_keys(0), genomic_heavy(0), has_genomic_breakpoints(false), n_tags(0), tag_csr_n(0), tag_csr_pairs(0), has_tags(false), has_tag_csr(false), blacklist_heavy(0), known_heavy(0), tags_heavy(0), dom_records(0), has_protein_domains(false) {
 	default_params(params);
 	memset(&timings, 0, sizeof(timings));
 	cons_rows = 0; cons_seq_bytes = cons_pos_count = cons_clip_bytes = 0;
@@ -109,6 +109,7 @@ void engine::set_contig_flags(const u8* flags, u32 n) { // per-sample flags (int
 void engine::set_annotation(const arb_annotation& a) {
 	if (has_contigs && a.n_contigs != annot.n_contigs) throw arb_error("annotation and contig table disagree on the number of contigs");
 	annot.n_genes = a.n_genes; annot.n_exons = a.n_exons; annot.n_contigs = a.n_contigs;
+	has_protein_domains = false; // the tables refer to genes of the annotation they were built on
 	annot.gene_contig.upload(ex, a.gene_contig, a.n_genes); annot.gene_start.upload(ex, a.gene_start, a.n_genes); annot.gene_end.upload(ex, a.gene_end, a.n_genes);
 	annot.gene_strand.upload(ex, a.gene_strand, a.n_genes); annot.gene_exonic_length.upload(ex, a.gene_exonic_length, a.n_genes); annot.gene_flags.upload(ex, a.gene_flags, a.n_genes);
 	annot.exon_gene.upload(ex, a.exon_gene, a.n_exons); annot.exon_start.upload(ex, a.exon_start, a.n_exons); annot.exon_end.upload(ex, a.exon_end, a.n_exons);

@@ -200,6 +200,13 @@ public:
 	u64 annotate_tags(u32 n_ids, const u32* ids, i32 max_mate_gap); void get_tags(u32* off, u32* ranks);
 	dbuf<u32> tag_rank_of_rule, tag_text_off, tag_csr_off, tag_csr_rank; dbuf<char> tag_text; u32 n_tags, tag_csr_n; u64 tag_csr_pairs; bool has_tags, has_tag_csr;
 	u32 blacklist_heavy, known_heavy, tags_heavy;
+	// protein domains (-p, protein_domains.cu): the per-gene table of domains_hd.h, dropped when the annotation is replaced; the retained_protein_domains
+	// column of the rows the host formats
+	void set_protein_domains(u32 n, const u16* contig, const i32* start, const i32* end, const u32* gene, const u32* name_rank, u32 n_names, const char* chars, const u32* off);
+	u64 retained_protein_domains(u32 n_ids, const u32* ids); void get_retained_protein_domains(u64* off, char* text);
+	struct domain_view domain_tables(); void check_domain_error(const char* who);
+	dbuf<u16> dom_contig; dbuf<i32> dom_start, dom_end; dbuf<u32> dom_mult, dom_name, dom_gene_off, dom_name_off, dom_error; dbuf<char> dom_name_chars, dom_text;
+	std::vector<u64> dom_text_off; u32 dom_records; bool has_protein_domains;
 private:
 	read_filter_params make_filter_params();
 	unsigned long genome_size() const;

@@ -1,6 +1,6 @@
 // cli_main.cpp -- the `arriba` command line of arriba-b200: same option letters, defaults and error texts as the reference
 // (options.cpp:270-485, usage options.cpp:109-268), driving the pipeline through the public C ABI only.
-// Not supported (fail loudly): -c Chimeric.out.sam, -p protein domains, -G, -I.
+// Not supported (fail loudly): -c Chimeric.out.sam, -G, -I.
 #include <getopt.h>
 #include <unistd.h>
 #include <sys/resource.h>
@@ -41,6 +41,7 @@ static void usage() {
 	          << " -i/-v contig lists, -E e-value cutoff, -S min support, -m/-L/-H/-R/-A/-M/-K/-V/-F/-U/-Q/-e/-l/-z/-Z thresholds as in the reference\n"
 	          << " -b FILE  blacklist (optionally .gz; required unless '-f blacklist')\n"
 	          << " -k FILE  known fusions (optionally .gz)   -t FILE  tags (optionally .gz)\n"
+	          << " -p FILE  protein domains (GFF3, optionally .gz)\n"
 	          << " -d FILE  genomic breakpoints from whole-genome sequencing (four-column or VCF, optionally .gz)\n -D N     maximum genomic breakpoint distance (default 100000)\n"
 	          << " -@ N     host threads for decoding and annotation   -u external duplicate marking   -X extra info for discarded candidates\n";
 }
@@ -52,7 +53,7 @@ int main(int argc, char** argv) {
 	o.echo_progress = 1;
 	o.threads = (int) std::max(1u, std::min(32u, std::thread::hardware_concurrency()));
 	crash(argc > 1 && (std::string(argv[1]).empty() || argv[1][0] != '-'), std::string("cannot interpret the first argument: ") + argv[1]);
-	std::string bam, gtf, fasta, out, discarded, interesting, viral, blacklist, genomic, known_fusions, tags;
+	std::string bam, gtf, fasta, out, discarded, interesting, viral, blacklist, genomic, known_fusions, tags, protein_domains;
 	opterr = 0;
 	const std::string valid = "c:x:d:g:G:o:O:t:p:a:b:k:s:i:v:f:E:S:m:L:H:D:R:A:M:K:V:F:U:Q:e:T:C:l:z:Z:@:uXIh";
 	std::map<char, unsigned> seen; int c; long iv; bool threads_given = false;
@@ -70,7 +71,8 @@ int main(int argc, char** argv) {
 			case 'D': crash(!int_in(optarg, 0, INT_MAX, iv), "invalid argument to " + opt); o.max_genomic_breakpoint_distance = (uint32_t) iv; break;
 			case 'k': known_fusions = optarg; crash(access(optarg, R_OK), "file not found/readable: " + known_fusions); break;
 			case 't': tags = optarg; crash(access(optarg, R_OK), "file not found/readable: " + tags); break;
-			case 'c': case 'p': case 'G': case 'I':
+			case 'p': protein_domains = optarg; crash(access(optarg, R_OK), "file not found/readable: " + protein_domains); break;
+			case 'c': case 'G': case 'I':
 				crash(true, "option " + opt + " is not supported by arriba-b200 (see DESIGN.md, out of scope)"); break;
 			case 's': { const std::string m = optarg; o.strandedness = m == "auto" ? 3 : m == "yes" ? 1 : m == "no" ? 0 : m == "reverse" ? 2 : -1; crash(o.strandedness < 0, "invalid type of strandedness: " + m); break; }
 			case 'i': interesting = optarg; std::replace(interesting.begin(), interesting.end(), ',', ' '); break;
@@ -124,6 +126,7 @@ int main(int argc, char** argv) {
 	o.genomic_breakpoints_file = genomic.empty() ? NULL : genomic.c_str();
 	o.blacklist_file = blacklist.empty() ? NULL : blacklist.c_str();
 	o.known_fusions_file = known_fusions.empty() ? NULL : known_fusions.c_str(); o.tags_file = tags.empty() ? NULL : tags.c_str();
+	o.protein_domains_file = protein_domains.empty() ? NULL : protein_domains.c_str();
 
 	arb_pipeline* p = NULL;
 	crash(arb_pipeline_create(&p, &o) != 0, arb_pipeline_error(NULL));

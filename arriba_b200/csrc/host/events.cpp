@@ -838,6 +838,40 @@ std::string pipeline::tags_of(u32 k) const {
 	return out;
 }
 
+// ------------------------------------------------------------------------------------------- protein domains (-p)
+// load_protein_domains (annotate_protein_domains.cpp:33-121): the records go to the device, which keeps the reference's index as a table per gene and fills
+// the retained_protein_domains column of the rows it formats (arb_format_discarded_rows) and, here, of the rows the host formats: those of fusions.tsv and,
+// with -X, the discarded ones.
+void pipeline::load_protein_domains() {
+	say("Loading protein domains from '" + opt.protein_domains_file + "'");
+	protein_domain_records r;
+	read_protein_domains(opt.protein_domains_file, ref, r);
+	std::vector<char> chars; std::vector<u32> off(1, 0);
+	for (size_t x = 0; x < r.names.size(); ++x) { chars.insert(chars.end(), r.names[x].begin(), r.names[x].end()); off.push_back((u32) chars.size()); }
+	chars.push_back(0);
+	check(ctx, arb_set_protein_domains(ctx, (uint32_t) r.contig.size(), r.contig.data(), r.start.data(), r.end.data(), r.gene.data(), r.name_rank.data(),
+	                                   (uint32_t) r.names.size(), chars.data(), off.data()), "arb_set_protein_domains");
+	const bool fusions = !opt.output_file.empty(), extra = !opt.discarded_output_file.empty() && opt.print_extra_info_for_discarded_fusions;
+	std::vector<u32> ids;
+	for (u32 k = 0; k < ev.n; ++k) if (ev.filter[k] == F_none ? fusions : extra) ids.push_back(k);
+	uint64_t bytes = 0;
+	if (arb_retained_protein_domains(ctx, (uint32_t) ids.size(), ids.data(), &bytes) != 0)
+		throw std::runtime_error("protein domains '" + opt.protein_domains_file + "': " + arb_last_error(ctx));
+	std::vector<u64> text_off(ids.size() + 1);
+	domain_text.assign(bytes + 1, 0);
+	check(ctx, arb_get_retained_protein_domains(ctx, text_off.data(), domain_text.data()), "arb_get_retained_protein_domains");
+	domain_off.assign((size_t) ev.n + 1, 0); // ids ascend: the texts lie in candidate order
+	for (size_t x = 0; x < ids.size(); ++x) domain_off[ids[x] + 1] = text_off[x + 1] - text_off[x];
+	for (u32 k = 0; k < ev.n; ++k) domain_off[k + 1] += domain_off[k];
+	domains_loaded = true;
+}
+
+// the retained_protein_domains column of candidate k, as the device formatted it
+std::string pipeline::domains_of(u32 k) const {
+	if (!domains_loaded || domain_off[k] == domain_off[k + 1]) return ".";
+	return std::string(domain_text.data() + domain_off[k], domain_off[k + 1] - domain_off[k]);
+}
+
 void pipeline::assign_confidence() { // filter_genomic_support.cpp:222-402
 	// the candidates of every gene (only counted below, so their order does not matter): one CSR table instead of a vector per gene
 	struct gene_list { const u32* p; size_t n; size_t size() const { return n; } u32 operator[](size_t x) const { return p[x]; } };

@@ -57,4 +57,10 @@ enum rule_file { RULES_BLACKLIST = 0, RULES_KNOWN_FUSIONS = 1, RULES_TAGS = 2 };
 void read_fusion_rules(const std::string& path, const refdata& ref, rule_file kind, i32 max_mate_gap, fusion_rules& out);
 void rank_tags(const fusion_rules& r, std::vector<std::string>& distinct, std::vector<u32>& rank);
 
+// protein domains of a GFF3 file (protein_domains.cpp), the accepted records in file order: contig, 0-based start and end, gene, and the rank of the decoded
+// name among the distinct names (bytewise order). Lines it rejects print the reference's WARNING on stderr; no accepted line, or a record the reference's index
+// cannot hold (contig id >= number of records), stops the run.
+struct protein_domain_records { std::vector<u16> contig; std::vector<i32> start, end; std::vector<u32> gene, name_rank; std::vector<std::string> names; };
+void read_protein_domains(const std::string& path, const refdata& ref, protein_domain_records& out);
+
 }} // namespace

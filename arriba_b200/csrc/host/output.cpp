@@ -718,7 +718,7 @@ struct writer {
 			    << ref.original_names[c5] << ":" << (b5 + 1) << "\t" << ref.original_names[c3] << ":" << (b3 + 1) << "\t" << site5 << "\t" << site3 << "\t"
 			    << fusion_type(k) << "\t" << s5 << "\t" << s3 << "\t" << e.discordant_mates[k] << "\t"
 			    << (cov5 >= 0 ? std::to_string((long long) cov5) : ".") << "\t" << (cov3 >= 0 ? std::to_string((long long) cov3) : ".") << "\t" << CONF[e.confidence[k] & 3] << "\t" << frame
-			    << "\t" << p.tags_of(k) << "\t.\t" << genomic_breakpoint(c5, b5, gb5) << "\t" << genomic_breakpoint(c3, b3, gb3);
+			    << "\t" << p.tags_of(k) << "\t" << p.domains_of(k) << "\t" << genomic_breakpoint(c5, b5, gb5) << "\t" << genomic_breakpoint(c3, b3, gb3);
 			// filters column: the candidate's own filter and, with counts, the filters of its supporting reads, in alphabetical order (output_fusions.cpp:1187-1213)
 			unsigned int filter_count[38]; bool filter_present[38];
 			for (int f = 0; f < 38; ++f) { filter_count[f] = 0; filter_present[f] = false; }
@@ -952,6 +952,7 @@ void pipeline::write_output() {
 	// files are opened and announced in the reference's order (output_fusions.cpp:1043, arriba.cpp:601-612)
 	int fd_fusions = -1, fd_discarded = -1;
 	if (!opt.tags_file.empty() && (fusions || discarded)) annotate_tags(); // arriba.cpp:591-595: the tags are loaded before any output file is opened
+	if (!opt.protein_domains_file.empty() && (fusions || discarded)) load_protein_domains(); // arriba.cpp:597-602: the protein domains after the tags
 	if (fusions) fd_fusions = writer::open_output(opt.output_file);
 	if (discarded) { try { fd_discarded = writer::open_output(opt.discarded_output_file); } catch (...) { if (fd_fusions >= 0) ::close(fd_fusions); throw; } }
 	writer::formatted text_fusions, text_discarded;

@@ -37,6 +37,7 @@ struct run_options { // options_t (options.hpp:25-69) restricted to what this im
 	std::string genomic_breakpoints_file; unsigned max_genomic_breakpoint_distance; // -d (empty: none), -D 100000
 	std::string blacklist_file; // -b (empty: none)
 	std::string known_fusions_file, tags_file; // -k, -t (empty: none)
+	std::string protein_domains_file; // -p (empty: none)
 	run_options();
 };
 
@@ -75,6 +76,8 @@ struct pipeline {
 	void recover_known_fusions(); // -k (recover_known_fusions.cpp)
 	void annotate_tags(); std::string tags_of(u32 k) const; // -t (annotate_tags.cpp): the tags of every written row, ranks per candidate
 	std::vector<std::string> tag_names; std::vector<u32> tag_off, tag_ranks; bool tags_loaded = false;
+	void load_protein_domains(); std::string domains_of(u32 k) const; // -p (annotate_protein_domains.cpp): the tables go to the device, which formats the column
+	std::vector<u64> domain_off; std::vector<char> domain_text; bool domains_loaded = false; // the column of the rows the host formats, per candidate
 	void write_output();
 	void make_kmer_index(); void filter_homologs(); void filter_mismappers(); bool splice_sites_ready;
 	void find_top_expressed_genes(std::vector<u32>& reads_by_gene, std::vector<u8>& present, unsigned int& threshold, float quantile);

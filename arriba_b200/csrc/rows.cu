@@ -51,6 +51,7 @@ void engine::format_discarded_rows(const u8* confidence, u64* n_rows, u64* n_byt
 	const bool tags = has_tag_csr && tag_csr_n == C; // arb_annotate_tags ran on this candidate table
 	fm.t.tag_text.chars = tags ? tag_text.ptr() : NULL; fm.t.tag_text.off = tags ? tag_text_off.ptr() : NULL;
 	fm.t.tag_off = tags ? tag_csr_off.ptr() : NULL; fm.t.tag_rank = tags ? tag_csr_rank.ptr() : NULL;
+	fm.t.domains = domain_tables();
 	for (int k = 0; k < ARB_N_FILTERS; ++k) fm.t.filters_by_name[k] = row_filters_by_name[k];
 	fm.t.max_itd_length = row_max_itd_length;
 	fm.l1o = cands.list1_off.ptr(); fm.l1 = cands.list1.ptr(); fm.l2o = cands.list2_off.ptr(); fm.l2 = cands.list2.ptr(); fm.ldo = cands.listd_off.ptr(); fm.ld = cands.listd.ptr();
@@ -70,6 +71,7 @@ void engine::format_discarded_rows(const u8* confidence, u64* n_rows, u64* n_byt
 		u32 total = 0; length.download(ex, &total, 1, STRIDE * b + n);
 		base[b + 1] = base[b] + total;
 	}
+	if (has_protein_domains) check_domain_error("arb_format_discarded_rows");
 	row_text.ensure(base[n_blocks] + 1);
 	for (u32 b = 0; b < n_blocks; ++b) {
 		const u32 lo = b * BLOCK, n = std::min(BLOCK, R - lo);

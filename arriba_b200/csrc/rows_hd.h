@@ -10,6 +10,7 @@
 #include "model.h"
 #include "annot_hd.h"
 #include "events_hd.h"
+#include "domains_hd.h"
 
 namespace arb {
 
@@ -22,6 +23,7 @@ struct row_tables { // what the rows need besides the candidate state, the fragm
 	const i32* closest1; const i32* closest2;      // closest genomic breakpoints per candidate (-d), NULL: none marked
 	coverage_view cov;
 	text_pool tag_text; const u32* tag_off; const u32* tag_rank; // -t: distinct tags by rank, and the ranks of every candidate's tags (CSR); NULL: no tags
+	domain_view domains;                           // -p: the protein domains per gene (domains_hd.h); gene_off NULL: none
 	u8 filters_by_name[ARB_N_FILTERS];             // filter ids in alphabetical order of their names
 	u32 max_itd_length;
 };
@@ -150,6 +152,48 @@ struct row_formatter {
 		for (u32 x = t.tag_off[k]; x < t.tag_off[k + 1]; ++x) { if (x > t.tag_off[k]) w.put(','); put_pool(w, t.tag_text, t.tag_rank[x]); }
 	}
 
+	// annotate_retained_protein_domains (annotate_protein_domains.cpp:123-161) for one side: its gene's records on its contig, per name (bytewise order) the
+	// lengths and the retained bases, each record counted mult times; "name(P%)" for every name with retained bases, joined by ','. Sums wrap like unsigned int.
+	template <class W> ARB_HD void domain_side(W& w, u32 gene, u32 contig, i32 bp, u32 dir, bool strand, bool ambiguous) const {
+		const domain_view& d = t.domains;
+		if (!coding(gene) || ambiguous || strand != forward(gene) || contig >= d.n_records) return;
+		bool any = false;
+		for (u32 x = d.gene_off[gene], last = d.gene_off[gene + 1]; x < last; ) {
+			const u32 name = d.name[x]; u32 length = 0, retained = 0;
+			for (; x < last && d.name[x] == name; ++x) {
+				if (d.contig[x] != contig) continue;
+				const i32 s = d.start[x], e = d.end[x]; const u32 m = d.mult[x];
+				u32 r = 0;
+				if (dir == UPSTREAM && e >= bp) r = (u32) e - (u32) (s > bp ? s : bp) + 1u;
+				else if (dir == DOWNSTREAM && s <= bp) r = (u32) (e < bp ? e : bp) - (u32) s + 1u;
+				length += m * ((u32) e - (u32) s + 1u); retained += m * r;
+			}
+			if (retained == 0) continue;
+			if (length == 0 && d.error) *d.error = 1u; // the reference divides by zero; the caller stops the run
+			if (any) w.put(',');
+			put_pool(w, text_pool{d.name_chars, d.name_off}, name); w.put('('); put_int(w, (long long) (length ? retained * 100u / length : 0u)); w.put('%'); w.put(')');
+			any = true;
+		}
+	}
+	// the retained_protein_domains column of candidate k (output_fusions.cpp:1183-1190): "p5|p3" if a side has any, else "."
+	template <class W> ARB_HD void retained_protein_domains(W& w, u32 k) const {
+		if (!t.domains.gene_off) { w.put('.'); return; }
+		const u8 bits = c.bits[k];
+		const bool ambiguous = bits & CB_PSTRANDS_AMBIGUOUS, first = bits & CB_TSTART_GENE1;
+		const u32 g5 = first ? c.gene1[k] : c.gene2[k], g3 = first ? c.gene2[k] : c.gene1[k], c5 = first ? c.contig1[k] : c.contig2[k], c3 = first ? c.contig2[k] : c.contig1[k];
+		const u32 d5 = first ? c.dir1[k] : c.dir2[k], d3 = first ? c.dir2[k] : c.dir1[k];
+		const i32 b5 = first ? c.bp1[k] : c.bp2[k], b3 = first ? c.bp2[k] : c.bp1[k];
+		const bool st1 = bits & CB_PSTRAND1, st2 = bits & CB_PSTRAND2, st5 = first ? st1 : st2, st3 = first ? st2 : st1;
+		count_writer n5 = {0}, n3 = {0};
+		domain_side(n5, g5, c5, b5, d5, st5, ambiguous); domain_side(n3, g3, c3, b3, d3, st3, ambiguous);
+		if (n5.n + n3.n == 0) { w.put('.'); return; }
+		both_sides(w, n5.n + n3.n + 1, g5, c5, b5, d5, st5, g3, c3, b3, d3, st3, ambiguous);
+	}
+	template <class W> ARB_HD void both_sides(W& w, u32, u32 g5, u32 c5, i32 b5, u32 d5, bool st5, u32 g3, u32 c3, i32 b3, u32 d3, bool st3, bool ambiguous) const {
+		domain_side(w, g5, c5, b5, d5, st5, ambiguous); w.put('|'); domain_side(w, g3, c3, b3, d3, st3, ambiguous);
+	}
+	ARB_HD void both_sides(count_writer& w, u32 n, u32, u32, i32, u32, bool, u32, u32, i32, u32, bool, bool) const { w.n += n; } // the length is known already
+
 	template <class W> ARB_HD void row(W& w, u32 k) const {
 		const u8 bits = c.bits[k];
 		u32 site5 = site(c.gene1[k], bits & CB_SPLICED1, bits & CB_EXONIC1, c.contig1[k], c.bp1[k]), site3 = site(c.gene2[k], bits & CB_SPLICED2, bits & CB_EXONIC2, c.contig2[k], c.bp2[k]);
@@ -170,7 +214,9 @@ struct row_formatter {
 		switch (t.confidence[k] & 3) { case 0: put_text(w, "low"); break; case 1: put_text(w, "medium"); break; default: put_text(w, "high"); break; }
 		put_text(w, "\t.\t"); // reading frame
 		tags(w, k);
-		put_text(w, "\t.\t"); // retained protein domains
+		w.put('\t');
+		retained_protein_domains(w, k);
+		w.put('\t');
 		genomic_breakpoint(w, c5, b5, gb5); w.put('\t'); genomic_breakpoint(w, c3, b3, gb3);
 		u32 count[ARB_N_FILTERS]; u64 present = 0;
 		for (u32 x = 0; x < ARB_N_FILTERS; ++x) count[x] = 0;
@@ -201,5 +247,8 @@ struct row_gather_fn { const u32* order; const u32* flag_scan; u32* rows; ARB_HD
 struct row_length_fn { row_formatter fm; const u32* rows; u32* length; ARB_HD void operator()(u32 x) const { count_writer w = {0}; fm.row(w, rows[x]); length[x] = w.n; } };
 // rows are written in blocks of a few million (a 10 M-fragment sample already has 0.8 GB of discarded rows: 32-bit offsets only inside a block)
 struct row_write_fn { row_formatter fm; const u32* rows; const u32* offset; char* text; ARB_HD void operator()(u32 x) const { memory_writer w = {text + offset[x]}; fm.row(w, rows[x]); } };
+// the retained_protein_domains column alone, for the rows the host formats (arb_retained_protein_domains)
+struct domain_length_fn { row_formatter fm; const u32* ids; u32* length; ARB_HD void operator()(u32 x) const { count_writer w = {0}; fm.retained_protein_domains(w, ids[x]); length[x] = w.n; } };
+struct domain_write_fn { row_formatter fm; const u32* ids; const u64* offset; char* text; ARB_HD void operator()(u32 x) const { memory_writer w = {text + offset[x]}; fm.retained_protein_domains(w, ids[x]); } };
 
 } // namespace arb

@@ -67,7 +67,7 @@ class Timings(C.Structure):
                 ("mismappers_pass1_ms", C.c_float), ("mismappers_pass2_ms", C.c_float), ("mismapper_tasks", C.c_uint64), ("mismapper_rounds", C.c_uint32), ("mismapper_overflow", C.c_uint32), ("mismapper_table_slots", C.c_uint32),
                 ("cascade_head_ms", C.c_float), ("cascade_sequences_ms", C.c_float), ("cascade_queued", C.c_uint64), ("cascade_algorithmic_bytes", C.c_uint64 * 2), ("annotate_ms", C.c_float), ("in_vitro_ms", C.c_float), ("multimappers_ms", C.c_float), ("order_ms", C.c_float), ("partners_ms", C.c_float), ("rows_ms", C.c_float), ("bam_scan_ms", C.c_float), ("consensus_ms", C.c_float), ("mismapper_algorithmic_bytes", C.c_uint64), ("mismapper_sequences", C.c_uint64), ("mismapper_hits", C.c_uint64),
                 ("genomic_support_ms", C.c_float), ("blacklist_ms", C.c_float), ("known_fusions_ms", C.c_float), ("tags_ms", C.c_float),
-                ("tags_match_ms", C.c_float), ("tags_sort_ms", C.c_float), ("tags_pairs", C.c_uint64)]
+                ("tags_match_ms", C.c_float), ("tags_sort_ms", C.c_float), ("tags_pairs", C.c_uint64), ("protein_domains_ms", C.c_float)]
 
 
 _CTYPE = {np.dtype(np.uint8): C.c_uint8, np.dtype(np.uint16): C.c_uint16, np.dtype(np.uint32): C.c_uint32, np.dtype(np.int32): C.c_int32,
@@ -137,6 +137,9 @@ def load(path=None):
                        ("arb_set_tags", [C.c_uint32] + [_p(C.c_uint8)] * 4 + [_p(C.c_uint16)] * 2 + [_p(C.c_int32)] * 4 + [_p(C.c_uint32)] * 2 + [_p(C.c_uint32), C.c_uint32, C.c_char_p, _p(C.c_uint32)]),
                        ("arb_annotate_tags", [C.c_uint32, _p(C.c_uint32), C.c_int32, _p(C.c_uint64)]),
                        ("arb_get_tags", [_p(C.c_uint32), _p(C.c_uint32)]),
+                       ("arb_set_protein_domains", [C.c_uint32, _p(C.c_uint16), _p(C.c_int32), _p(C.c_int32), _p(C.c_uint32), _p(C.c_uint32), C.c_uint32, C.c_char_p, _p(C.c_uint32)]),
+                       ("arb_retained_protein_domains", [C.c_uint32, _p(C.c_uint32), _p(C.c_uint64)]),
+                       ("arb_get_retained_protein_domains", [_p(C.c_uint64), C.c_char_p]),
                        ("arb_set_candidate_state", [_p(C.c_uint8), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_float)]),
                        ("arb_set_candidate_lists", [_p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32)]),
                        ("arb_set_splice_sites", [_p(C.c_uint32), _p(C.c_int32)]),
@@ -403,6 +406,32 @@ class Context:
         self._check(self.lib.arb_get_tags(self.h, ptr(off), ptr(ranks)))
         return [[self._tag_names[r] for r in ranks[off[k]:off[k + 1]]] for k in range(n)]
 
+    # ---- protein domains (-p)
+    def set_protein_domains(self, contig, start, end, gene, names):
+        """The accepted records of a GFF3 file in file order: contig, 0-based start and end, gene, and the decoded name (bytes or str) of every record."""
+        cols = [np.ascontiguousarray(contig, np.uint16), np.ascontiguousarray(start, np.int32), np.ascontiguousarray(end, np.int32), np.ascontiguousarray(gene, np.uint32)]
+        names = [t.encode("latin-1") if isinstance(t, str) else bytes(t) for t in names]
+        n = cols[0].size
+        assert all(c.size == n for c in cols) and len(names) == n, "columns differ in length"
+        distinct = sorted(set(names))
+        index = {t: k for k, t in enumerate(distinct)}
+        rank = np.array([index[t] for t in names] if n else [0], np.uint32)
+        off = np.zeros(len(distinct) + 1, np.uint32); off[1:] = np.cumsum([len(t) for t in distinct]) if distinct else []
+        chars = b"".join(distinct) + b"\0"
+        self._keep.append(chars)
+        cols = [c if c.size else np.zeros(1, c.dtype) for c in cols]
+        self._check(self.lib.arb_set_protein_domains(self.h, n, *[ptr(c) for c in cols], ptr(rank), len(distinct), chars, ptr(off)))
+
+    def retained_protein_domains(self, ids):
+        """The retained_protein_domains column (bytes, "." when empty) of every candidate in `ids`, from the tables of set_protein_domains."""
+        ids = np.ascontiguousarray(ids, np.uint32)
+        nbytes = C.c_uint64()
+        self._check(self.lib.arb_retained_protein_domains(self.h, ids.size, ptr(ids if ids.size else np.zeros(1, np.uint32)), C.byref(nbytes)))
+        off = np.zeros(ids.size + 1, np.uint64); text = C.create_string_buffer(int(nbytes.value) + 1)
+        self._check(self.lib.arb_get_retained_protein_domains(self.h, ptr(off), text))
+        raw = text.raw
+        return [raw[int(off[x]):int(off[x + 1])] for x in range(ids.size)]
+
     def slot_swaps(self):
         s = np.zeros(self.n_fragments, np.uint8)
         self._check(self.lib.arb_get_slot_swaps(self.h, ptr(s)))
@@ -466,7 +495,7 @@ class RunOptions(C.Structure):
                 ("print_extra_info_for_discarded_fusions", C.c_int32), ("echo_progress", C.c_int32),
                 ("top_viral_contigs", C.c_uint32), ("viral_contig_min_covered_fraction", C.c_float),
                 ("genomic_breakpoints_file", C.c_char_p), ("max_genomic_breakpoint_distance", C.c_uint32), ("blacklist_file", C.c_char_p),
-                ("known_fusions_file", C.c_char_p), ("tags_file", C.c_char_p)]
+                ("known_fusions_file", C.c_char_p), ("tags_file", C.c_char_p), ("protein_domains_file", C.c_char_p)]
 
 
 class RunStats(C.Structure):
@@ -512,7 +541,7 @@ class Pipeline:
     """One run of the hot path on files: the call a user of the library makes (the `arriba` CLI is a thin wrapper over it)."""
 
     def __init__(self, bam, gtf, fasta, threads=1, device=0, lib_path=None, strandedness=3, params=None, output=None, discarded=None,
-                 genomic_breakpoints=None, max_genomic_breakpoint_distance=100000, blacklist=None, known_fusions=None, tags=None):
+                 genomic_breakpoints=None, max_genomic_breakpoint_distance=100000, blacklist=None, known_fusions=None, tags=None, protein_domains=None):
         self.lib = load(lib_path)
         _load_pipeline_api(self.lib)
         o = RunOptions()
@@ -532,6 +561,8 @@ class Pipeline:
             self._strings.append(known_fusions.encode()); o.known_fusions_file = self._strings[-1]
         if tags:
             self._strings.append(tags.encode()); o.tags_file = self._strings[-1]
+        if protein_domains:
+            self._strings.append(protein_domains.encode()); o.protein_domains_file = self._strings[-1]
         o.threads = threads; o.device = device; o.strandedness = strandedness
         if params is not None:
             o.params = params

@@ -373,6 +373,19 @@ int arb_set_tags(arb_ctx* ctx, uint32_t n, const uint8_t* type1, const uint8_t* 
 int arb_annotate_tags(arb_ctx* ctx, uint32_t n_ids, const uint32_t* ids, int32_t max_mate_gap, uint64_t* n_pairs);
 int arb_get_tags(arb_ctx* ctx, uint32_t* off, uint32_t* ranks);
 
+/* ---- protein domains (-p) ---------------------------------------------------------------------------------------------------------------------------------
+ * arb_set_protein_domains replaces the index of load_protein_domains (source/annotate_protein_domains.cpp:33-121, make_annotation_index in
+ * annotation.t.hpp:25-45): the n accepted records of the GFF3 file in file order, 0-based (contig < n, gene: its gene, name_rank < n_names: the rank of its
+ * decoded name among the distinct names in bytewise order), and the texts of the n_names names in that order (name k = name_chars[name_off[k] .. name_off[k + 1])).
+ * The tables stay on the device until the annotation is replaced; arb_format_discarded_rows fills the retained_protein_domains column from them.
+ * arb_retained_protein_domains formats that column (annotate_retained_protein_domains for both sides, output_fusions.cpp:1183-1190: "p5|p3" or ".") for the
+ * candidates `ids`; *n_bytes is the size of all texts. arb_get_retained_protein_domains returns them: off[n_ids + 1] and the texts, id x at text[off[x] .. off[x + 1]).
+ * A domain name whose summed length wraps to 0 while its retained bases do not (the reference divides by zero) stops either call with an error. */
+int arb_set_protein_domains(arb_ctx* ctx, uint32_t n, const uint16_t* contig, const int32_t* start, const int32_t* end, const uint32_t* gene, const uint32_t* name_rank,
+                            uint32_t n_names, const char* name_chars, const uint32_t* name_off);
+int arb_retained_protein_domains(arb_ctx* ctx, uint32_t n_ids, const uint32_t* ids, uint64_t* n_bytes);
+int arb_get_retained_protein_domains(arb_ctx* ctx, uint64_t* off, char* text);
+
 /* ---- device timing (CUDA events recorded on the context's stream around each stage) ---------------------------------- */
 typedef struct arb_timings {
 	float duplicates_ms;        /* duplicate marking (key build + hash group-by + mark) */
@@ -408,6 +421,7 @@ typedef struct arb_timings {
 	float tags_match_ms;        /* arb_annotate_tags, its first part: key table of the rules and both passes over the rows */
 	float tags_sort_ms;         /* arb_annotate_tags, its second part: sort of the (row, tag) pairs, duplicates removed, the per-candidate table */
 	uint64_t tags_pairs;        /* arb_annotate_tags: (row, matching rule) pairs before duplicates are removed (a rule counts once per bin it is met in) */
+	float protein_domains_ms;   /* arb_set_protein_domains (sort of the index keys, multiplicities, per-gene table) plus every arb_retained_protein_domains since */
 } arb_timings;
 int arb_get_timings(arb_ctx* ctx, arb_timings* out);
 /* Device scratch memory is pooled per device and survives arb_ctx_destroy so that the next sample reuses it; this returns it to the driver
@@ -451,6 +465,7 @@ typedef struct arb_run_options {
 	const char* blacklist_file;      /* -b: blacklist rules (optionally .gz), NULL = none; read only while the blacklist filter is on */
 	const char* known_fusions_file;  /* -k: known fusions (optionally .gz), NULL = none; read only while the known_fusions filter is on */
 	const char* tags_file;           /* -t: tags (optionally .gz), NULL = none */
+	const char* protein_domains_file; /* -p: protein domains (GFF3, optionally .gz), NULL = none */
 } arb_run_options;
 void arb_default_run_options(arb_run_options* o);
 
