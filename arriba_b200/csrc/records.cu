@@ -3,8 +3,9 @@
 //   records_chunk  : per chunk of inflated payload: copy it up behind the unfinished record of the previous chunk, find the records (bamscan.cu), classify
 //                    them and append the kept ones to the record store, which lives across chunks (mates and supplementaries of one key may sit anywhere
 //                    in the file),
-//   records_finish : sort the store by key hash (two stable 32-bit passes: file order inside a hash), replay every run of equal hashes (count, scan,
-//                    write) into the fragment pools that fragment_table_build reads, and bring the coverage windows and the counters back.
+//   records_finish : sort the store by key hash (two stable 32-bit passes: file order inside a hash), replay every run of equal hashes (count and log
+//                    the searches' outcomes, scan, write from the log) into the fragment pools that fragment_table_build reads, saturate the coverage
+//                    counts into packed 16-bit windows, and bring the windows and the counters back.
 #include <cstdlib>
 #include <cstdio>
 #include "engine.h"
@@ -25,6 +26,15 @@ template <class T> static void grow_keep(const exec_ctx& ex, dbuf<T>& b, size_t 
 #endif
 	}
 	b.swap(bigger);
+}
+
+// n items from the device to the host, queued on the stream (the caller synchronises)
+template <class T> static void copy_to_host(const exec_ctx& ex, T* host, const T* dev, size_t n) {
+#ifdef ARB_DEVICE_BUILD
+	ARB_CUDA_CHECK(cudaMemcpyAsync(host, dev, n * sizeof(T), cudaMemcpyDeviceToHost, ex.stream));
+#else
+	(void) ex; memcpy(host, dev, n * sizeof(T));
+#endif
 }
 
 void engine::records_begin(const u16* tid_to_contig, u32 n_tid, const u8* interesting, const u8* viral, const u64* n_windows, u32 n_contigs,
@@ -48,12 +58,13 @@ void engine::records_begin(const u16* tid_to_contig, u32 n_tid, const u8* intere
 	const char* bits = getenv("ARB_KEY_HASH_BITS");
 	rec_hash_mask = bits && atoi(bits) > 0 && atoi(bits) < 64 ? ((u64) 1 << atoi(bits)) - 1 : ~(u64) 0;
 	timings.bam_scan_ms = 0; timings.h2d_ms = 0; timings.h2d_bytes = 0;
+	timings.rec_chunk_copy_ms = timings.rec_chunk_kernels_ms = timings.rec_sort_ms = timings.rec_count_ms = timings.rec_scan_ms = timings.rec_write_ms = timings.rec_download_ms = 0;
 	rec_open = true;
 }
 
 void engine::records_chunk(const u8* chunk, u64 bytes, u64 first, u64 chunk_pos, u64* n_records, u64* carry, u32* malformed, u64* error) {
 	if (!rec_open) throw arb_error("arb_records_chunk without arb_records_begin");
-	stage_timer t_all(ex);
+	stage_timer t_all(ex), t_copy(ex);
 	// the unfinished record at the end of the previous chunk goes in front of this one
 	const u64 total = rec_carry + bytes;
 	if (total >= 0xFFFFFFF0ull) throw arb_error("failed to load alignments (chunk too large)");
@@ -67,13 +78,15 @@ void engine::records_chunk(const u8* chunk, u64 bytes, u64 first, u64 chunk_pos,
 	}
 	bam_buf_next.upload_at(ex, chunk, bytes, rec_carry);
 	bam_buf.swap(bam_buf_next);
+	timings.rec_chunk_copy_ms += t_copy.stop();
+	stage_timer t_kernels(ex);
 	const u64 buf_pos = chunk_pos - rec_carry;
 	u64 consumed = 0; u32 R = 0;
 	dbuf<u32> rec_off;
 	bam_scan(bam_buf.ptr(), total, rec_carry ? 0 : first, (i32) rec_n_tid, rec_off, &consumed, &R, malformed);
 	*n_records = R;
 	rec_carry_at = consumed; rec_carry = total - consumed; *carry = rec_carry;
-	if (*malformed || R == 0) { rec_error.download(ex, error, 1); timings.bam_scan_ms += t_all.stop(); return; }
+	if (*malformed || R == 0) { rec_error.download(ex, error, 1); timings.rec_chunk_kernels_ms += t_kernels.stop(); timings.bam_scan_ms += t_all.stop(); return; }
 	// classify, then append the kept records to the store
 	dbuf<u32> bytes_of((size_t) R + 1), kept((size_t) R + 1); dbuf<u64> hash(R); dbuf<i64> hit(R); dbuf<u8> sa(R);
 	const rec_chunk_view cv = {bam_buf.ptr(), rec_off.ptr(), buf_pos, rec_tid.ptr(), (i32) rec_n_tid, annot.contig_len.ptr(), rec_interesting.ptr()};
@@ -113,6 +126,7 @@ void engine::records_chunk(const u8* chunk, u64 bytes, u64 first, u64 chunk_pos,
 			rec_error_record.resize(n); bam_buf.download(ex, rec_error_record.data(), n, at - buf_pos + 4);
 		}
 	}
+	timings.rec_chunk_kernels_ms += t_kernels.stop();
 	timings.bam_scan_ms += t_all.stop();
 }
 
@@ -128,7 +142,7 @@ struct rec_iota_fn { u32* v; ARB_HD void operator()(u32 k) const { v[k] = k; } }
 void engine::records_finish(u16* const* coverage, u8* const* starts, u8* const* ends, u64* counters, u64* error) {
 	if (!rec_open) throw arb_error("arb_records_finish without arb_records_begin");
 	rec_open = false;
-	stage_timer t_all(ex);
+	stage_timer t_all(ex), t_sort(ex);
 	const u32 n = (u32) rec_n;
 	// 1. key order: low word, then high word, both stable (file order inside a key hash)
 	dbuf<u32> order((size_t) n + 1), key((size_t) n + 1), tk((size_t) n + 1), tv((size_t) n + 1);
@@ -144,23 +158,28 @@ void engine::records_finish(u16* const* coverage, u8* const* starts, u8* const* 
 	u32 S = 0; seg_at.download(ex, &S, 1, n);
 	dbuf<u32> seg_begin((size_t) S + 1);
 	rec_seg_begin_fn bf = {seg_at.ptr(), n, seg_begin.ptr()}; for_each(ex, n + 1, bf);
-	// 3. replay: count (sets of 32 gene ids, the few segments that need more: 1024), scan, write
+	timings.rec_sort_ms = t_sort.stop();
+	stage_timer t_count(ex);
+	// 3. replay: count (sets of up to 32 gene ids, the few segments that need more: 1024), scan, write
 	dbuf<u8> big((size_t) S + 1); big.zero(ex, (size_t) S + 1);
 	const u32 stride = (S + 4) & ~3u; // S + 1 entries per row, rows 16-byte aligned (the scan loads four items at a time)
 	dbuf<u32> tally((size_t) RS_N * stride), big_list((size_t) S + 1), n_big(1);
+	dbuf<u64> search_log((size_t) n + 1); // what the counting pass's searches decided, per store position (written before it is read: no zeroing)
 	const rec_store_view sv = {rec_arena.ptr(), rec_at.ptr(), rec_pos.ptr(), rec_hit.ptr(), rec_sa.ptr(), order.ptr()};
-	const rec_cov_view cov = {rec_cov_words.ptr(), rec_cov_starts.ptr(), rec_cov_ends.ptr(), rec_cov_off.ptr(), rec_cov_n.ptr(), rec_n_contigs};
+	rec_cov_view cov = {NULL, rec_cov_starts.ptr(), rec_cov_ends.ptr(), rec_cov_off.ptr(), rec_cov_n.ptr(), rec_n_contigs}; // counts: writing pass only
 	const rec_params prm = {rec_max_itd, (u8) (rec_external_dup ? 1 : 0), rec_viral.ptr()};
 	const annot_view an = annot.view();
-	rec_replay_fn<32> small = {sv, seg_begin.ptr(), NULL, big.ptr(), an, prm, cov, tally.ptr(), tally.ptr(), stride, NULL, NULL, NULL, NULL, NULL, rec_counters.ptr(), rec_error.ptr(), false};
+	rec_replay_fn<32> small = {sv, seg_begin.ptr(), NULL, big.ptr(), an, prm, cov, tally.ptr(), tally.ptr(), stride, NULL, NULL, NULL, NULL, NULL, search_log.ptr(), rec_counters.ptr(), rec_error.ptr(), false};
 	for_each(ex, S, small);
 	n_big.zero(ex, 1);
 	rec_big_list_fn lf = {big.ptr(), big_list.ptr(), n_big.ptr()}; for_each(ex, S, lf);
 	u32 B = 0; n_big.download(ex, &B, 1);
-	rec_replay_fn<1024> large = {sv, seg_begin.ptr(), big_list.ptr(), big.ptr(), an, prm, cov, tally.ptr(), tally.ptr(), stride, NULL, NULL, NULL, NULL, NULL, rec_counters.ptr(), rec_error.ptr(), false};
+	rec_replay_fn<1024> large = {sv, seg_begin.ptr(), big_list.ptr(), big.ptr(), an, prm, cov, tally.ptr(), tally.ptr(), stride, NULL, NULL, NULL, NULL, NULL, search_log.ptr(), rec_counters.ptr(), rec_error.ptr(), false};
 	for_each(ex, B, large);
 	rec_error.download(ex, error, 1);
+	timings.rec_count_ms = t_count.stop();
 	if (*error != ~(u64) 0) { timings.bam_scan_ms += t_all.stop(); return; }
+	stage_timer t_scan(ex);
 	// The scans are 32-bit. A prefix sum that passes 2^32 wraps, and every wrap shows as a step down between neighbours (each tally is < 2^32): counted,
 	// the true totals follow, and a sample whose pools the table cannot address stops here, before anything is written.
 	for (u32 q = 0; q < RS_N; ++q) exclusive_scan_u32(ex, tally.ptr() + (size_t) q * stride, tally.ptr() + (size_t) q * stride, S);
@@ -169,6 +188,7 @@ void engine::records_finish(u16* const* coverage, u8* const* starts, u8* const* 
 	u32 tot[RS_N], n_wraps[RS_N];
 	for (u32 q = 0; q < RS_N; ++q) tally.download(ex, tot + q, 1, (size_t) q * stride + S);
 	wraps.download(ex, n_wraps, RS_N);
+	timings.rec_scan_ms = t_scan.stop();
 	{
 		u64 total[RS_N], limit[RS_N] = {(u64) 1 << 30 /* fragment ids */, (u64) 1 << 31 /* i32 alignment links */, (u64) 1 << 32, (u64) 1 << 32, (u64) 1 << 32};
 		const char* hook = getenv("ARB_REPLAY_POOL_LIMIT"); // test hook: the limits lowered, so that a small sample reaches them
@@ -188,8 +208,11 @@ void engine::records_finish(u16* const* coverage, u8* const* starts, u8* const* 
 			throw arb_error(m);
 		}
 	}
+	stage_timer t_write(ex);
 	pool_frags.ensure(tot[RS_FRAGS]); pool_alns.ensure(tot[RS_ALNS]); pool_names.ensure(tot[RS_NAMES]); pool_cigars.ensure(tot[RS_CIGARS]); pool_seqs.ensure((size_t) tot[RS_UNITS] * 16);
+	dbuf<u64> cov_counts(rec_cov_windows + 2); cov_counts.zero(ex, rec_cov_windows + 2);
 	small.write = large.write = true;
+	small.cov.counts = large.cov.counts = cov_counts.ptr();
 	small.frags = large.frags = pool_frags.ptr(); small.alns = large.alns = pool_alns.ptr(); small.names = large.names = pool_names.ptr();
 	small.cigars = large.cigars = pool_cigars.ptr(); small.seqs = large.seqs = pool_seqs.ptr();
 	for_each(ex, S, small);
@@ -197,19 +220,21 @@ void engine::records_finish(u16* const* coverage, u8* const* starts, u8* const* 
 	const u64 base[2 * FT_POOLS] = {0, tot[RS_FRAGS], 0, tot[RS_ALNS], 0, tot[RS_NAMES], 0, tot[RS_CIGARS], 0, (u64) tot[RS_UNITS] * 16};
 	pool_base.upload(ex, base, 2 * FT_POOLS);
 	pool_workers = 1;
-	// 4. the by-products
+	timings.rec_write_ms = t_write.stop();
+	stage_timer t_download(ex);
+	// 4. the by-products: the counts saturated into packed 16-bit windows, then every contig's windows straight into the caller's arrays (the
+	// 16-bit counters lie in their 32-bit words in little-endian order, i.e. as a plain u16 array)
+	rec_cov_pack_fn pk = {cov_counts.ptr(), rec_cov_words.ptr()}; for_each(ex, (u32) (rec_cov_windows / 2 + 1), pk);
 	std::vector<u64> off((size_t) rec_n_contigs + 1); rec_cov_off.download(ex, off.data(), off.size());
-	// three bulk copies; the 16-bit counters lie in their 32-bit words in little-endian order, i.e. as a plain u16 array
-	std::vector<u16> windows(rec_cov_windows + 2); std::vector<u8> fs(rec_cov_windows + 1), fe(rec_cov_windows + 1);
-	rec_cov_words.download(ex, (u32*) windows.data(), rec_cov_windows / 2 + 1);
-	rec_cov_starts.download(ex, fs.data(), rec_cov_windows); rec_cov_ends.download(ex, fe.data(), rec_cov_windows);
+	const u16* windows = (const u16*) rec_cov_words.ptr();
 	for (u32 c = 0; c < rec_n_contigs; ++c) {
 		const u64 w = off[c + 1] - off[c];
 		if (!w) continue;
-		memcpy(coverage[c], windows.data() + off[c], w * 2); memcpy(starts[c], fs.data() + off[c], w); memcpy(ends[c], fe.data() + off[c], w);
+		copy_to_host(ex, coverage[c], windows + off[c], w); copy_to_host(ex, starts[c], rec_cov_starts.ptr() + off[c], w); copy_to_host(ex, ends[c], rec_cov_ends.ptr() + off[c], w);
 	}
-	rec_counters.download(ex, counters, (size_t) REC_CTR_VIRAL + rec_n_contigs);
+	rec_counters.download(ex, counters, (size_t) REC_CTR_VIRAL + rec_n_contigs); // synchronises: the copies above are done
 	rec_error.download(ex, error, 1);
+	timings.rec_download_ms = t_download.stop();
 	// the store is not needed any more: its memory goes to the fragment table
 	rec_arena.release(); rec_at.release(); rec_pos.release(); rec_hash_lo.release(); rec_hash_hi.release(); rec_hit.release(); rec_sa.release(); bam_buf_next.release();
 	timings.bam_scan_ms += t_all.stop();

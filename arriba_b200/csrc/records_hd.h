@@ -6,7 +6,10 @@
 //   rec_replay_fn  : one thread per run of equal key hashes (the store sorted stably by hash: file order inside a run): every key of the run replays the
 //                    loop's steps in file order -- supplementaries, discordant mates, proper pairs (each record alternates between waiting and pairing),
 //                    tandem duplications in soft clips, split reads, read-through fragments, pristine viral reads, coverage -- once to count what it
-//                    emits, once to write the fragment pools (the layout fragtable.cu reads, one pool).
+//                    emits, once to write the fragment pools (the layout fragtable.cu reads, one pool). The searches (the genome scan for tandem
+//                    duplications, the gene-index queries of the read-through test) run in the counting pass only: it logs what they decided per record,
+//                    and the writing pass replays from that log,
+//   rec_cov_pack_fn: the coverage counts of the writing pass, saturated to 16 bits and packed two to a 32-bit word.
 #pragma once
 #include "model.h"
 #include "prims.h"
@@ -35,6 +38,36 @@ ARB_HD void rec_atomic_add_u64(u64* p, u64 v) {
 	atomicAdd((unsigned long long*) p, (unsigned long long) v);
 #else
 	*p += v;
+#endif
+}
+// aligned 8- and 16-byte stores: a thread that copies a record byte by byte issues one store per byte, to lines no other lane of its warp touches
+ARB_HD void rec_put_u64(u8* d /* 8-byte aligned */, u64 v) {
+#ifdef __CUDA_ARCH__
+	*(u64*) d = v;
+#else
+	memcpy(d, &v, 8);
+#endif
+}
+ARB_HD void rec_put_u128(u8* d /* 16-byte aligned */, u64 lo, u64 hi) {
+#ifdef __CUDA_ARCH__
+	*(ulonglong2*) d = make_ulonglong2(lo, hi);
+#else
+	memcpy(d, &lo, 8); memcpy(d + 8, &hi, 8);
+#endif
+}
+// bytes [at, at + 8) of src as a little-endian word, zero from byte n on
+ARB_HD u64 rec_get_u64(const u8* src, u32 at, u32 n) {
+	u64 v = 0;
+	for (u32 x = 0; x < 8; ++x) if (at + x < n) v |= (u64) src[at + x] << (8 * x);
+	return v;
+}
+// +1 on a counter that every thread of a launch may bump: on the device one atomic per warp (the active lanes' increments summed)
+ARB_HD void rec_count_one(u64* p) {
+#ifdef __CUDA_ARCH__
+	const unsigned active = __activemask();
+	if ((threadIdx.x & 31u) == (unsigned) __ffs((int) active) - 1u) atomicAdd((unsigned long long*) p, (unsigned long long) __popc(active));
+#else
+	*p += 1;
 #endif
 }
 
@@ -151,13 +184,13 @@ struct rec_extract_fn {
 		i64 hit_index = 1;
 		const u8* hi = rec_find_aux(r, 'H', 'I');
 		if (hi) hit_index = rec_aux_int(hi);
-		else if (r.flag & BF_SECONDARY) { rec_atomic_add_u64(&counters[REC_CTR_MISSING_HI], 1); return; }
+		else if (r.flag & BF_SECONDARY) { rec_count_one(&counters[REC_CTR_MISSING_HI]); return; }
 		if (r.tid < 0 || r.tid >= c.n_tid) { fail(i, REC_ERR_LOAD); return; }
 		const u32 contig = c.tid_to_contig[r.tid];
 		i64 query_span;
 		const u32 bad = rec_validate(r, c.contig_len[contig], query_span);
 		if (bad) { fail(i, bad); return; }
-		if (!(r.flag & BF_SUPPLEMENTARY) && c.interesting[contig]) rec_atomic_add_u64(&counters[REC_CTR_MAPPED], 1);
+		if (!(r.flag & BF_SUPPLEMENTARY) && c.interesting[contig]) rec_count_one(&counters[REC_CTR_MAPPED]);
 		bytes[i] = r.compact_bytes(); kept[i] = 1;
 		hash[i] = rec_key_hash(r.qname(), r.name_len(), hit_index) & hash_mask; hit[i] = hit_index;
 		has_sa[i] = rec_find_aux(r, 'S', 'A') != 0;
@@ -171,13 +204,11 @@ struct rec_store_fn { // record i of the chunk -> store item n_stored + kept[i] 
 		const u8* p = c.B + c.rec_off[i] + 4;
 		const u64 k = n_stored + kept[i], dst = arena_used + at[i], size = at[i + 1] - at[i];
 		rec_t r; rec_parse(p, rec_rd32(p - 4), r);
-		const u32 head = 32u + r.l_qname + 4u * r.n_cigar, n_seq = ((u32) r.l_seq + 1) / 2;
-		u8* d = arena + dst;
-		for (u32 b = 0; b < head; ++b) d[b] = p[b];
-		for (u32 b = 0; b < n_seq; ++b) d[head + b] = r.seq[b];
-		for (u32 b = head + n_seq; b < size; ++b) d[b] = 0;
+		const u32 head = 32u + r.l_qname + 4u * r.n_cigar, n_seq = ((u32) r.l_seq + 1) / 2; // the sequence follows the CIGAR: p[0, head + n_seq)
+		u8* d = arena + dst; // 8-byte aligned, `size` a multiple of 8
 		const u32 contig = c.tid_to_contig[r.tid];
-		d[0] = (u8) contig; d[1] = (u8) (contig >> 8); d[2] = 0; d[3] = 0;
+		rec_put_u64(d, (rec_get_u64(p, 0, head + n_seq) & ~(u64) 0xFFFFFFFFu) | contig); // the contig id in place of the BAM's reference id
+		for (u32 b = 8; b < size; b += 8) rec_put_u64(d + b, rec_get_u64(p, b, head + n_seq));
 		s_at[k] = dst; s_pos[k] = c.buf_pos + c.rec_off[i]; s_hash_lo[k] = (u32) hash[i]; s_hash_hi[k] = (u32) (hash[i] >> 32); s_hit[k] = hit[i]; s_sa[k] = has_sa[i];
 	}
 };
@@ -196,7 +227,7 @@ struct rec_store_view {
 		return true;
 	}
 };
-struct rec_cov_view { u32* words /* u16 counters, two per word */; u8* starts; u8* ends; const u64* off; const u32* n; u32 n_contigs; };
+struct rec_cov_view { u64* counts /* per window; packed by rec_cov_pack_fn */; u8* starts; u8* ends; const u64* off; const u32* n; u32 n_contigs; };
 struct rec_params { u32 max_itd_length; u8 external_duplicate_marking; const u8* viral; };
 // per segment: fragments, alignments, name bytes, CIGAR operations, 16-byte sequence units; exclusive scans of them turn into the segments' write bases
 enum { RS_FRAGS = 0, RS_ALNS = 1, RS_NAMES = 2, RS_CIGARS = 3, RS_UNITS = 4, RS_N = 5 };
@@ -344,7 +375,7 @@ struct rec_emit {
 	ARB_HD u64 store_seq(const rec_t& r) { // nt16 nibbles copied verbatim, 16-byte aligned, the rest of the last unit zero
 		const u32 bytes = ((u32) r.l_seq + 1) / 2, units = (bytes + 15) / 16;
 		const u64 off = (u64) (base[RS_UNITS] + n[RS_UNITS]) * 16;
-		if (writing()) { u8* d = seqs + off; for (u32 b = 0; b < units * 16; ++b) d[b] = b < bytes ? r.seq[b] : 0; }
+		if (writing()) for (u32 u = 0; u < units; ++u) rec_put_u128(seqs + off + 16 * u, rec_get_u64(r.seq, 16 * u, bytes), rec_get_u64(r.seq, 16 * u + 8, bytes));
 		n[RS_UNITS] += units;
 		return off;
 	}
@@ -384,17 +415,16 @@ struct rec_emit {
 	}
 };
 
-// coverage (read_stats.cpp:161-266): saturating 16-bit counters, two to a 32-bit word
-ARB_HD void cov_increment(u32* words, u64 w) {
-	u32* word = words + (w >> 1); const u32 sh = (u32) (w & 1) * 16;
-	u32 seen = *(volatile u32*) word;
-	for (;;) {
-		if ((seen >> sh & 0xFFFFu) == 0xFFFFu) return;
-		const u32 prev = atomic_cas_u32(word, seen, seen + (1u << sh));
-		if (prev == seen) return;
-		seen = prev;
+// coverage (read_stats.cpp:161-266): the reference's counters are 16 bits wide and saturate. Saturating increments commute -- the final value is
+// min(increments, 65535) in any order -- so the writing pass adds plainly into 64-bit counts (which no sample can wrap) and rec_cov_pack_fn saturates.
+ARB_HD void cov_increment(u64* counts, u64 w) { rec_atomic_add_u64(counts + w, 1); }
+struct rec_cov_pack_fn { // word i: windows 2i (low half) and 2i + 1 (high half), as a plain little-endian u16 array
+	const u64* counts; u32* words;
+	ARB_HD void operator()(u32 i) const {
+		const u64 a = counts[2 * (u64) i], b = counts[2 * (u64) i + 1];
+		words[i] = (u32) (a < 0xFFFFu ? a : 0xFFFFu) | (u32) (b < 0xFFFFu ? b : 0xFFFFu) << 16;
 	}
-}
+};
 ARB_HD void add_coverage(const rec_cov_view& cov, const rec_t& m1, const rec_t* m2p, bool is_chimeric, bool flags_cleared) {
 	const rec_t& m2 = m2p ? *m2p : m1;
 	const u32 f1 = flags_cleared ? 0 : m1.flag;
@@ -418,7 +448,7 @@ ARB_HD void add_coverage(const rec_cov_view& cov, const rec_t& m1, const rec_t* 
 		const bool consumes_query = o == C_M || o == C_I || o == C_S || o == C_EQ || o == C_X;
 		if (consumes_query) {
 			while (window <= position / 20) {
-				if (position - window * 20 >= 10) cov_increment(cov.words, cov.off[contig] + (u64) window);
+				if (position - window * 20 >= 10) cov_increment(cov.counts, cov.off[contig] + (u64) window);
 				++window;
 			}
 		} else window = position / 20;
@@ -428,31 +458,51 @@ ARB_HD void add_coverage(const rec_cov_view& cov, const rec_t& m1, const rec_t* 
 	}
 }
 
-// One thread per segment (run of equal key hashes). The set capacity CAP bounds the gene sets of the read-through test: a segment whose sets overflow CAP
-// is left untouched and marked in `big` for a second launch with the reference's capacity (1024), where an overflow is the reference's fatal error.
-// Counting pass (write == false): the segment's tallies. Writing pass: the pools, the coverage, the counters.
+// What the counting pass decided for a record that reached the searches, indexed by store position (the writing pass replays from it):
+//   bits 0-1: the tandem duplication found in the record's / its mate's soft clip (REC_LOG_TANDEM_*),
+//   bits 2-3: the read-through branch taken (REC_RT_*), bits 4-5: the forward / reverse mate spans an intron at the gene boundary,
+//   bits 16-31 / 32-47: the CIGAR operation of that intron in the forward / reverse mate (an index below n_cigar, which is 16 bits wide).
+enum { REC_LOG_TANDEM_RECORD = 1, REC_LOG_TANDEM_MATE = 2, REC_LOG_RT_SHIFT = 2, REC_LOG_F_INTRON = 16, REC_LOG_R_INTRON = 32 };
+enum { REC_RT_NONE = 0, REC_RT_FORWARD_INTRON = 1, REC_RT_REVERSE_INTRON = 2, REC_RT_INSIDE = 3 };
+ARB_HD u64 rec_log_read_through(u32 branch, bool f_intron, bool r_intron, u32 fop, u32 rop) {
+	return (u64) branch << REC_LOG_RT_SHIFT | (f_intron ? REC_LOG_F_INTRON : 0) | (r_intron ? REC_LOG_R_INTRON : 0) | (u64) (fop & 0xFFFFu) << 16 | (u64) (rop & 0xFFFFu) << 32;
+}
+
+// the gene ids that a point query of the gene index returns (query_index with start == end): the item list of one region, or none
+struct rec_genes { const u32* v; u32 n; };
+ARB_HD rec_genes rec_genes_at(const region_index_view& ix, u32 contig, i32 pos) {
+	rec_genes g = {0, 0};
+	if (contig >= ix.n_contigs) return g;
+	const u32 lo = ix.begin[contig], hi = ix.begin[contig + 1];
+	const u32 r = region_find(ix, contig, lo, hi, pos);
+	if (r < hi) { g.v = ix.items + ix.off[r]; g.n = ix.off[r + 1] - ix.off[r]; }
+	return g;
+}
+
+// One thread per segment (run of equal key hashes). CAP bounds the gene sets of the read-through test, as the reference's fixed-capacity sets do: a segment
+// whose sets exceed 32 ids is left untouched and marked in `big` for a second launch with the reference's capacity (1024), where more is the reference's
+// fatal error. The sets are read in place from the gene index; CAP only decides which launch a segment belongs to.
+// Counting pass (write == false): the searches, their log, the segment's tallies. Writing pass: the pools, the coverage, the counters.
 template <int CAP> struct rec_replay_fn {
 	rec_store_view s; const u32* seg_begin; const u32* list /* segments of this launch, NULL: all */; u8* big;
 	annot_view an; rec_params prm; rec_cov_view cov;
 	u32* tally /* RS_N rows of `stride` entries, one per segment */; const u32* bases /* the rows after their exclusive scans */; u32 stride;
 	arb_pool_fragment* frags; arb_pool_alignment* alns; char* names; u32* cigars; u8* seqs;
-	u64* counters; u64* error; bool write;
+	u64* log /* per store position: what the searches decided */; u64* counters; u64* error; bool write;
 
-	// read-through fragments (read_chimeric_alignments.cpp:93-193); returns false and marks the segment when a gene set overflows CAP
-	ARB_HD bool extract_read_through(rec_emit& e, u32 k, i64 hit_index, const rec_t* a, const rec_t* b, bool& is_read_through) const {
-		is_read_through = false;
+	// the decision of the read-through test (read_chimeric_alignments.cpp:93-193) as a log entry; returns false and marks the segment when a gene set exceeds CAP
+	ARB_HD bool decide_read_through(u32 k, const rec_t* a, const rec_t* b, u64& decision) const {
+		decision = 0;
 		const rec_t* fm = a; const rec_t* rm = b;
 		if (fm->reverse()) { const rec_t* t = fm; fm = rm; rm = t; }
-		idset<CAP> fg, rg, common;
 		const region_index_view gix = gene_index(an);
-		if (fm) query_index(gix, (u32) fm->tid, fm->pos, fm->pos, fg); else query_index(gix, (u32) rm->tid, rm->pos, rm->pos, fg);
-		if (rm) query_index(gix, (u32) rm->tid, rm->endpos(), rm->endpos(), rg); else query_index(gix, (u32) fm->tid, fm->endpos(), fm->endpos(), rg);
-		if (fg.overflow || rg.overflow) {
+		const rec_genes fg = fm ? rec_genes_at(gix, (u32) fm->tid, fm->pos) : rec_genes_at(gix, (u32) rm->tid, rm->pos);
+		const rec_genes rg = rm ? rec_genes_at(gix, (u32) rm->tid, rm->endpos()) : rec_genes_at(gix, (u32) fm->tid, fm->endpos());
+		if (fg.n > (u32) CAP || rg.n > (u32) CAP) {
 			if (CAP >= 1024) rec_atomic_min_u64(error, s.pos[k] << 3 | REC_ERR_ANNOTATION);
 			return false;
 		}
-		combine_sets(fg.v, fg.n, rg.v, rg.n, common, false);
-		if (!(common.n == 0 && !(fg.n == 0 && rg.n == 0))) return true;
+		if (sets_intersect(fg.v, fg.n, rg.v, rg.n) || (fg.n == 0 && rg.n == 0)) return true;
 		i32 fgs, fge, rgs, rge;
 		gene_set_extent(an, fg.v, fg.n, fgs, fge); gene_set_extent(an, rg.v, rg.n, rgs, rge);
 		if (fge == -1) fge = rgs - 1;
@@ -460,28 +510,33 @@ template <int CAP> struct rec_replay_fn {
 		u32 fop = 0, rop = 0; i32 fpos = 0, rpos = 0;
 		const bool f_intron = fm ? spanning_intron(*fm, fge, rgs, fop, fpos) : false;
 		const bool r_intron = rm ? spanning_intron(*rm, fge, rgs, rop, rpos) : false;
+		u32 branch = REC_RT_NONE;
+		if (f_intron && (!r_intron || fpos < rm->l_seq - rpos)) branch = REC_RT_FORWARD_INTRON;
+		else if (r_intron) branch = REC_RT_REVERSE_INTRON;
+		else if (fm && rm && rm->pos >= rgs && fm->endpos() <= fge) branch = REC_RT_INSIDE;
+		decision = rec_log_read_through(branch, f_intron, r_intron, fop, rop);
+		return true;
+	}
+	// the read-through fragment that `decision` calls for; returns whether the record is a read-through one
+	ARB_HD bool emit_read_through(rec_emit& e, i64 hit_index, const rec_t* a, const rec_t* b, u64 decision) const {
+		const rec_t* fm = a; const rec_t* rm = b;
+		if (fm->reverse()) { const rec_t* t = fm; fm = rm; rm = t; }
+		const u32 branch = (u32) (decision >> REC_LOG_RT_SHIFT) & 3u, fop = (u32) (decision >> 16) & 0xFFFFu, rop = (u32) (decision >> 32) & 0xFFFFu;
+		const bool f_intron = decision & REC_LOG_F_INTRON, r_intron = decision & REC_LOG_R_INTRON;
 		const rec_t& named = *a;
-		if (f_intron && (!r_intron || fpos < rm->l_seq - rpos)) {
-			bool created; const u32 f = e.fragment(named, hit_index, 0, &created);
-			if (created) {
-				e.add_alignment(f, *fm, false, fop + 1, 1);
-				e.add_alignment(f, *fm, true, fop - 1, 2);
-				if (rm) { if (r_intron) e.add_alignment(f, *rm, false, rop + 1, 1); else e.add_alignment(f, *rm, false); }
-				is_read_through = true;
-			}
-		} else if (r_intron) {
-			bool created; const u32 f = e.fragment(named, hit_index, 0, &created);
-			if (created) {
-				e.add_alignment(f, *rm, true, rop + 1, 1);
-				e.add_alignment(f, *rm, false, rop - 1, 2);
-				if (fm) { if (f_intron) e.add_alignment(f, *fm, false, fop - 1, 2); else e.add_alignment(f, *fm, false); }
-				is_read_through = true;
-			}
-		} else if (fm && rm && rm->pos >= rgs && fm->endpos() <= fge) {
-			bool created; const u32 f = e.fragment(named, hit_index, 0, &created);
-			if (created) { e.add_alignment(f, *fm, false); e.add_alignment(f, *rm, false); }
-			is_read_through = true;
-		}
+		if (branch == REC_RT_NONE) return false;
+		bool created; const u32 f = e.fragment(named, hit_index, 0, &created);
+		if (branch == REC_RT_FORWARD_INTRON) {
+			if (!created) return false;
+			e.add_alignment(f, *fm, false, fop + 1, 1);
+			e.add_alignment(f, *fm, true, fop - 1, 2);
+			if (rm) { if (r_intron) e.add_alignment(f, *rm, false, rop + 1, 1); else e.add_alignment(f, *rm, false); }
+		} else if (branch == REC_RT_REVERSE_INTRON) {
+			if (!created) return false;
+			e.add_alignment(f, *rm, true, rop + 1, 1);
+			e.add_alignment(f, *rm, false, rop - 1, 2);
+			if (fm) { if (f_intron) e.add_alignment(f, *fm, false, fop - 1, 2); else e.add_alignment(f, *fm, false); }
+		} else if (created) { e.add_alignment(f, *fm, false); e.add_alignment(f, *rm, false); }
 		return true;
 	}
 
@@ -509,14 +564,17 @@ template <int CAP> struct rec_replay_fn {
 			mk = (u32) waiting; waiting = -1;
 			s.get(mk, mate); m = &mate;
 		}
-		bool is_tandem = false;
+		u64 decision = write ? log[k] : 0;
 		tandem_t t;
-		bool tandem_from_record = false, tandem_from_mate = false;
-		if (!clipped_sequence_is_adapter(r, m) && (!m || r.reverse() != m->reverse())) {
-			tandem_from_record = tandem_duplication(an, prm.max_itd_length, &r, t);
-			if (!tandem_from_record) tandem_from_mate = tandem_duplication(an, prm.max_itd_length, m, t);
-		}
-		if (tandem_from_record || tandem_from_mate) {
+		if (!write) {
+			if (!clipped_sequence_is_adapter(r, m) && (!m || r.reverse() != m->reverse())) {
+				if (tandem_duplication(an, prm.max_itd_length, &r, t)) decision = REC_LOG_TANDEM_RECORD;
+				else if (tandem_duplication(an, prm.max_itd_length, m, t)) decision = REC_LOG_TANDEM_MATE;
+			}
+		} else if (decision & REC_LOG_TANDEM_RECORD) tandem_duplication(an, prm.max_itd_length, &r, t); // a hit is rare: its search runs again to rebuild it
+		else if (decision & REC_LOG_TANDEM_MATE) tandem_duplication(an, prm.max_itd_length, m, t);
+		const bool tandem_from_mate = decision & REC_LOG_TANDEM_MATE, is_tandem = decision & (REC_LOG_TANDEM_RECORD | REC_LOG_TANDEM_MATE);
+		if (is_tandem) {
 			const u32 f = e.fragment(r, hit_index, 1, 0);
 			e.add_alignment(f, r, (!r.reverse()) == t.forward && !t.supplementary);
 			if (m) e.add_alignment(f, *m, (!m->reverse()) == t.forward && !t.supplementary);
@@ -525,7 +583,6 @@ template <int CAP> struct rec_replay_fn {
 			if (!t.supplementary) { const rec_t& src = tandem_from_mate ? *m : r; a.seq_off = e.store_seq(src); a.seq_len = (u32) src.l_seq; }
 			a.cigar_off = e.base[RS_CIGARS] + e.n[RS_CIGARS]; for (u32 x = 0; x < t.n_cigar; ++x) e.push_cigar(t.cigar[x]); a.cigar_cnt = t.n_cigar;
 			e.link(f, a);
-			is_tandem = true;
 		}
 		bool is_read_through = false;
 		if ((s.sa[k] && clipped_at_correct_end(r)) || (m && s.sa[mk] && clipped_at_correct_end(*m))) {
@@ -534,12 +591,18 @@ template <int CAP> struct rec_replay_fn {
 			if (m) e.add_alignment(f, *m, false);
 			if (write) counters[REC_CTR_CHIMERIC] = 1;
 		} else if (!is_tandem) {
-			if (!extract_read_through(e, k, hit_index, &r, m, is_read_through)) return false;
+			if (!write) {
+				u64 rt;
+				if (!decide_read_through(k, &r, m, rt)) return false;
+				decision |= rt;
+			}
+			is_read_through = emit_read_through(e, hit_index, &r, m, decision);
 			if (write && prm.viral[r.tid]) {
 				if (pristine(r)) rec_atomic_add_u64(&counters[REC_CTR_VIRAL + r.tid], 1);
 				if (m && pristine(*m)) rec_atomic_add_u64(&counters[REC_CTR_VIRAL + m->tid], 1);
 			}
 		}
+		if (!write) log[k] = decision;
 		if (write && (!prm.external_duplicate_marking || !(r.flag & BF_DUP))) add_coverage(cov, r, m, is_read_through, false);
 		return true;
 	}

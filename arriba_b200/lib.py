@@ -67,7 +67,9 @@ class Timings(C.Structure):
                 ("mismappers_pass1_ms", C.c_float), ("mismappers_pass2_ms", C.c_float), ("mismapper_tasks", C.c_uint64), ("mismapper_rounds", C.c_uint32), ("mismapper_overflow", C.c_uint32), ("mismapper_table_slots", C.c_uint32),
                 ("cascade_head_ms", C.c_float), ("cascade_sequences_ms", C.c_float), ("cascade_queued", C.c_uint64), ("cascade_algorithmic_bytes", C.c_uint64 * 2), ("annotate_ms", C.c_float), ("in_vitro_ms", C.c_float), ("multimappers_ms", C.c_float), ("order_ms", C.c_float), ("partners_ms", C.c_float), ("rows_ms", C.c_float), ("bam_scan_ms", C.c_float), ("consensus_ms", C.c_float), ("mismapper_algorithmic_bytes", C.c_uint64), ("mismapper_sequences", C.c_uint64), ("mismapper_hits", C.c_uint64),
                 ("genomic_support_ms", C.c_float), ("blacklist_ms", C.c_float), ("known_fusions_ms", C.c_float), ("tags_ms", C.c_float),
-                ("tags_match_ms", C.c_float), ("tags_sort_ms", C.c_float), ("tags_pairs", C.c_uint64), ("protein_domains_ms", C.c_float)]
+                ("tags_match_ms", C.c_float), ("tags_sort_ms", C.c_float), ("tags_pairs", C.c_uint64), ("protein_domains_ms", C.c_float),
+                ("rec_chunk_copy_ms", C.c_float), ("rec_chunk_kernels_ms", C.c_float), ("rec_sort_ms", C.c_float), ("rec_count_ms", C.c_float),
+                ("rec_scan_ms", C.c_float), ("rec_write_ms", C.c_float), ("rec_download_ms", C.c_float)]
 
 
 _CTYPE = {np.dtype(np.uint8): C.c_uint8, np.dtype(np.uint16): C.c_uint16, np.dtype(np.uint32): C.c_uint32, np.dtype(np.int32): C.c_int32,

@@ -422,6 +422,15 @@ typedef struct arb_timings {
 	float tags_sort_ms;         /* arb_annotate_tags, its second part: sort of the (row, tag) pairs, duplicates removed, the per-candidate table */
 	uint64_t tags_pairs;        /* arb_annotate_tags: (row, matching rule) pairs before duplicates are removed (a rule counts once per bin it is met in) */
 	float protein_domains_ms;   /* arb_set_protein_domains (sort of the index keys, multiplicities, per-gene table) plus every arb_retained_protein_domains since */
+	/* laps of bam_scan_ms. arb_records_chunk, summed over the chunks of the last sample: */
+	float rec_chunk_copy_ms;    /* the chunk (behind the carried unfinished record) copied to the device */
+	float rec_chunk_kernels_ms; /* record boundaries, classification, the scans of the sizes, store growth and the copy into the store */
+	/* arb_records_finish: */
+	float rec_sort_ms;          /* both radix passes over the key hashes (with their gathers) and the segment boundaries */
+	float rec_count_ms;         /* the counting replay launches (both set capacities) and the list of segments for the second one */
+	float rec_scan_ms;          /* the exclusive scans of the tallies, the wrap count and the download of the totals */
+	float rec_write_ms;         /* the writing replay launches (pools and coverage counts) */
+	float rec_download_ms;      /* the coverage windows packed and brought back with the counters */
 } arb_timings;
 int arb_get_timings(arb_ctx* ctx, arb_timings* out);
 /* Device scratch memory is pooled per device and survives arb_ctx_destroy so that the next sample reuses it; this returns it to the driver

@@ -1,0 +1,70 @@
+"""Where the BAM ingest of the cfg2 workload (bench.py's default world) spends its time: whole ingest steps through the public Pipeline API (the reference
+loaded outside the clock), a warm-up, then timed steps. One JSON line with the card's name and power limit, and per timed step:
+  - ingest_s and ingest_split (inflate / parse / finalize, host clocks, as bench.py reports them),
+  - bam_scan_ms and its laps (CUDA events, arb_timings.rec_*): per-chunk copy and kernels summed over the chunks; sort, counting launches, scans,
+    writing launches, coverage and counter download of arb_records_finish,
+  - finalize_rest_s: finalize less the device laps of arb_records_finish (the fragment-table build, its download and the host's share).
+Also the rate of a plain copy of one page-locked 128 MiB host buffer to the device in the same process: the PCIe floor of the chunk stream.
+
+python tools/ingest_bench.py [--warmup 1] [--steps 3] [--threads N]"""
+import argparse, json, os, statistics, sys, time
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import bench
+from arriba_b200 import lib as L, _build
+
+LAPS = ["rec_chunk_copy_ms", "rec_chunk_kernels_ms", "rec_sort_ms", "rec_count_ms", "rec_scan_ms", "rec_write_ms", "rec_download_ms"]
+
+
+def pinned_h2d_gbps(reps=10):
+    import torch
+    src = torch.empty(128 << 20, dtype=torch.uint8, pin_memory=True)
+    dst = torch.empty(128 << 20, dtype=torch.uint8, device="cuda")
+    dst.copy_(src, non_blocking=True); torch.cuda.synchronize()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(reps):
+        dst.copy_(src, non_blocking=True)
+    b.record(); b.synchronize()
+    return reps * (128 << 20) / (a.elapsed_time(b) * 1e-3) / 1e9
+
+
+def one_step(prefix, threads):
+    p = L.Pipeline(prefix + ".bam", prefix + ".gtf", prefix + ".fa", threads=threads)
+    p.step(L.STEP_LOAD_REFERENCE)
+    t0 = time.perf_counter()
+    p.step(L.STEP_INGEST)
+    ingest_s = time.perf_counter() - t0
+    s = p.stats(); t = p.context().timings()
+    laps = {k: round(getattr(t, k), 2) for k in LAPS}
+    finish_ms = sum(laps[k] for k in LAPS[2:])
+    r = {"ingest_s": round(ingest_s, 3), "ingest_split": {"inflate": round(s.t_inflate, 3), "parse": round(s.t_parse, 3), "finalize": round(s.t_finalize, 3)},
+         "bam_scan_ms": round(t.bam_scan_ms, 1), "laps_ms": laps, "finalize_rest_s": round(s.t_finalize - finish_ms * 1e-3, 3),
+         "records": int(s.n_records), "fragments": int(s.n_fragments)}
+    p.close()
+    return r
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--warmup", type=int, default=1); ap.add_argument("--steps", type=int, default=3)
+    ap.add_argument("--threads", type=int, default=2 * (len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else 8))
+    ap.add_argument("--workload", default="cfg2_10M_2x101_50k")
+    a = ap.parse_args()
+    if not os.path.exists(_build.PRODUCT_LIB):
+        _build.build_product()
+    prefix = bench.ensure_world(a.workload)
+    card = bench.ClockSampler(0).card()
+    for _ in range(a.warmup):
+        one_step(prefix, a.threads)
+    steps = [one_step(prefix, a.threads) for _ in range(a.steps)]
+    med = lambda f: statistics.median(f(r) for r in steps)
+    out = {"workload": a.workload, "threads": a.threads, **card, "pinned_h2d_128MiB_GBps": round(pinned_h2d_gbps(), 2),
+           "median": {"ingest_s": med(lambda r: r["ingest_s"]), "finalize_s": med(lambda r: r["ingest_split"]["finalize"]), "bam_scan_ms": med(lambda r: r["bam_scan_ms"]),
+                      "laps_ms": {k: med(lambda r: r["laps_ms"][k]) for k in LAPS}},
+           "steps": steps}
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()
