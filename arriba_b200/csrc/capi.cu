@@ -113,6 +113,12 @@ int arb_records_begin(arb_ctx* ctx, const uint16_t* tid_to_contig, uint32_t n_ti
 int arb_records_chunk(arb_ctx* ctx, const uint8_t* chunk, uint64_t bytes, uint64_t first, uint64_t chunk_pos, uint64_t* n_records, uint64_t* carry, uint32_t* malformed, uint64_t* error) {
 	ARB_API_BEGIN(ctx) u64 r = 0, c = 0, e = 0; ctx->e.records_chunk(chunk, bytes, first, chunk_pos, &r, &c, malformed, &e); *n_records = r; *carry = c; *error = e; ARB_API_END(ctx)
 }
+int arb_records_text_names(arb_ctx* ctx, const char* names, const uint64_t* name_off, uint32_t n_names) {
+	ARB_API_BEGIN(ctx) std::vector<u64> off(name_off, name_off + n_names + 1); ctx->e.records_text_names(names, off.data(), n_names); ARB_API_END(ctx)
+}
+int arb_records_text_chunk(arb_ctx* ctx, const uint8_t* chunk, uint64_t bytes, uint64_t first, uint64_t chunk_pos, int last, uint64_t* n_records, uint64_t* carry, uint64_t* error) {
+	ARB_API_BEGIN(ctx) u64 r = 0, c = 0, e = 0; ctx->e.records_text_chunk(chunk, bytes, first, chunk_pos, last != 0, &r, &c, &e); *n_records = r; *carry = c; *error = e; ARB_API_END(ctx)
+}
 int arb_records_error_record(arb_ctx* ctx, const uint8_t** body, uint64_t* bytes) {
 	ARB_API_BEGIN(ctx) *body = ctx->e.rec_error_record.data(); *bytes = ctx->e.rec_error_record.size(); ARB_API_END(ctx)
 }

@@ -150,6 +150,12 @@ public:
 	void records_begin(const u16* tid_to_contig, u32 n_tid, const u8* interesting, const u8* viral, const u64* n_windows, u32 n_contigs, u32 max_itd_length, bool external_duplicate_marking, u64 expected_bytes);
 	void records_chunk(const u8* chunk, u64 bytes, u64 first, u64 chunk_pos, u64* n_records, u64* carry, u32* malformed, u64* error);
 	void records_finish(u16* const* coverage, u8* const* starts, u8* const* ends, u64* counters, u64* error);
+	u64 records_upload(const u8* chunk, u64 bytes);
+	void records_store(const dbuf<u8>& B, u64 buf_pos, u64 total, const u32* rec_off, u32 R, u64 seen, u64* error);
+	// SAM text input (samscan.cu): lines staged as BAM records, then records_store
+	void records_text_names(const char* names, const u64* name_off, u32 n);
+	void records_text_chunk(const u8* chunk, u64 bytes, u64 first, u64 chunk_pos, bool last, u64* n_records, u64* carry, u64* error);
+	dbuf<u8> sam_blob, sam_stage; dbuf<u64> sam_name_off; dbuf<u32> sam_name_tid; u32 sam_n_names = 0; u64 rec_text_staged = 0;
 	dbuf<u8> rec_arena, rec_sa, rec_interesting, rec_viral, rec_cov_starts, rec_cov_ends; dbuf<u64> rec_at, rec_pos, rec_error, rec_counters, rec_cov_off; dbuf<i64> rec_hit;
 	dbuf<u32> rec_hash_lo, rec_hash_hi, rec_cov_words, rec_cov_n; dbuf<u16> rec_tid;
 	u64 rec_n, rec_arena_used, rec_carry, rec_carry_at, rec_expected_bytes, rec_cov_windows, rec_hash_mask; u32 rec_n_tid, rec_n_contigs, rec_max_itd; bool rec_external_dup, rec_open;

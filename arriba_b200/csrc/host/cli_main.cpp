@@ -36,7 +36,7 @@ static const char* FILTERS[] = {"", "duplicates", "inconsistently_clipped", "hom
 static void usage() {
 	std::cout << "arriba-b200: H100-native implementation of Arriba's post-alignment path (reference version 2.5.1 semantics)\n\n"
 	          << "Usage: arriba -x Aligned.out.bam -g annotation.gtf -a assembly.fa -o fusions.tsv [-O fusions.discarded.tsv] [OPTIONS]\n\n"
-	          << " -x FILE  BAM with main and chimeric alignments (STAR --chimOutType WithinBAM)\n -g FILE  gene annotation (GTF)\n -a FILE  assembly (FastA)\n"
+	          << " -x FILE  BAM or SAM (plain or BGZF) with main and chimeric alignments (STAR --chimOutType WithinBAM)\n -g FILE  gene annotation (GTF)\n -a FILE  assembly (FastA)\n"
 	          << " -o FILE  output file   -O FILE  discarded candidates\n -f LIST  disable filters (comma/space separated)\n -s MODE  strandedness auto|yes|no|reverse\n"
 	          << " -i/-v contig lists, -E e-value cutoff, -S min support, -m/-L/-H/-R/-A/-M/-K/-V/-F/-U/-Q/-e/-l/-z/-Z thresholds as in the reference\n"
 	          << " -b FILE  blacklist (optionally .gz; required unless '-f blacklist')\n"

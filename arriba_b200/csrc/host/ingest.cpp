@@ -1,4 +1,4 @@
-// ingest.cpp -- see ingest.h. BGZF blocks are inflated in parallel on the host and the header is read here; everything the reference's record loop does
+// ingest.cpp -- see ingest.h. BGZF blocks (or pieces of a plain SAM file) are copied into chunks in parallel on the host and the header (BAM, or SAM's @ lines) is read here; everything the reference's record loop does
 // runs on the device (csrc/records.cu), and so does the fragment table (csrc/fragtable.cu).
 #include "ingest.h"
 #include "../../../include/arriba_b200.h"
@@ -112,16 +112,25 @@ struct bgzf_file {
 	const u8* data; size_t size; int fd;
 	struct block { u64 in_off; u32 in_len; u32 out_len; u64 out_off; };
 	std::vector<block> blocks; u64 total_out;
-	bgzf_file(): data(NULL), size(0), fd(-1), total_out(0) {}
+	bgzf_file(): data(NULL), size(0), fd(-1), total_out(0), raw(false) {}
 	~bgzf_file() { if (data) munmap((void*) data, size); if (fd >= 0) close(fd); }
-	void open(const std::string& path, int threads) {
+	bool raw; // plain SAM text: the "blocks" are pieces of the file, copied as they are
+	void map(const std::string& path) {
 		fd = ::open(path.c_str(), O_RDONLY);
 		if (fd < 0) fail("failed to open SAM file");
 		struct stat st; fstat(fd, &st); size = st.st_size;
+		if (!S_ISREG(st.st_mode)) fail("failed to open SAM file (input from a pipe or device is not supported: pass a regular file)");
 		if (size == 0) fail("failed to read SAM header");
 		data = (const u8*) mmap(NULL, size, PROT_READ, MAP_PRIVATE, fd, 0);
 		if (data == MAP_FAILED) { data = NULL; fail("failed to open SAM file"); }
 		madvise((void*) data, size, MADV_SEQUENTIAL);
+	}
+	void raw_pieces(u64 piece) {
+		raw = true;
+		for (u64 off = 0; off < size; off += piece) { block b; b.in_off = b.out_off = off; b.in_len = b.out_len = (u32) std::min<u64>(piece, size - off); blocks.push_back(b); }
+		total_out = size;
+	}
+	void block_table(int threads) {
 		// Block table. A block is found from the one before it (its size sits in its header), and every header read faults a page of the mapping in: a
 		// 7 GB file of stored blocks costs a quarter of a second on one thread. So every piece of the file guesses its first block (two well-formed
 		// headers in a row), walks from there, and the guesses are VERIFIED: the chain of piece s must arrive exactly at the guess of piece s+1; where it
@@ -181,6 +190,7 @@ struct bgzf_file {
 	}
 	void inflate_block(const block& b, u8* dst) const {
 		if (b.out_len == 0) return;
+		if (raw) { memcpy(dst, data + b.in_off, b.out_len); return; }
 		// STAR is run with --outBAMcompression 0 (run_arriba.sh:34): every BGZF block then holds ONE stored deflate block -- header byte 0x01 (final, type 00),
 		// LEN, ~LEN, the bytes (RFC 1951 3.2.4). Those are copied; anything else goes through zlib.
 		const u8* const in = data + b.in_off;
@@ -233,19 +243,84 @@ static std::string record_error_text(u64 error, arb_ctx* ctx, const std::vector<
 	return "failed to load alignments";
 }
 
+// The format is decided by the file's content, as htslib's sam_open does: BGZF whose stream starts with "BAM\1" is BAM, any other BGZF stream is SAM
+// text, and a file that is not gzip is plain SAM if its first line starts with '@' or has at least 10 tabs. The block table is built here (BGZF), or the
+// file is cut into pieces of at most 4 MiB, and no larger than a chunk (but at least 256 bytes), that are copied as they are (plain SAM).
+enum input_format { INPUT_BAM, INPUT_SAM_BGZF, INPUT_SAM };
+static input_format detect_format(bgzf_file& f, int threads, u64 chunk_target) {
+	const u8* d = f.data;
+	if (f.size >= 3 && d[0] == 0x1f && d[1] == 0x8b && d[2] == 8) {
+		const u32 xlen = f.size >= 12 ? rd16(d + 10) : 0;
+		bool bgzf = false;
+		if ((d[3] & 4) && f.size >= 12ull + xlen)
+			for (u32 x = 0; x + 4 <= xlen;) { const u8* e = d + 12 + x; if (e[0] == 'B' && e[1] == 'C') bgzf = true; x += 4 + rd16(e + 2); }
+		if (!bgzf) fail("failed to read SAM header (gzip-compressed SAM must be BGZF (bgzip) or uncompressed)");
+		f.block_table(threads);
+		std::vector<u8> head;
+		for (size_t b = 0; b < f.blocks.size() && head.size() < 4; ++b) { const size_t at = head.size(); head.resize(at + f.blocks[b].out_len); f.inflate_block(f.blocks[b], head.data() + at); }
+		return head.size() >= 4 && memcmp(head.data(), "BAM\1", 4) == 0 ? INPUT_BAM : INPUT_SAM_BGZF;
+	}
+	if (f.size >= 4 && memcmp(d, "CRAM", 4) == 0) fail("failed to read SAM header (CRAM input is not supported: convert it to BAM or SAM)");
+	u32 tabs = 0;
+	for (size_t x = 0; x < f.size && d[x] != '\n'; ++x) tabs += d[x] == '\t';
+	if (d[0] != '@' && tabs < 10) fail("failed to read SAM header");
+	f.raw_pieces(std::max<u64>(256, std::min<u64>(chunk_target, 4ull << 20)));
+	return INPUT_SAM;
+}
+
+// The @ lines at the start of a SAM stream, however many blocks they span; every @SQ line gives the next reference (its SN) to `reference`. Returns the
+// offset of the first record in the stream.
+template <class F> static u64 read_sam_header(const bgzf_file& f, F reference) {
+	std::string text; size_t inflated = 0;
+	auto more = [&]() {
+		if (inflated >= f.blocks.size()) return false;
+		const size_t at = text.size(); text.resize(at + f.blocks[inflated].out_len); f.inflate_block(f.blocks[inflated], (u8*) &text[at]); ++inflated;
+		return true;
+	};
+	size_t p = 0;
+	for (;;) {
+		while (p >= text.size() && more()) {}
+		if (p >= text.size() || text[p] != '@') return p;
+		size_t lf;
+		while ((lf = text.find('\n', p)) == std::string::npos && more()) {}
+		std::string line = text.substr(p, lf == std::string::npos ? std::string::npos : lf - p);
+		if (lf != std::string::npos && !line.empty() && line.back() == '\r') line.pop_back();
+		if (line.compare(0, 4, "@SQ\t") == 0) {
+			std::string name; bool has_name = false, has_length = false;
+			for (size_t a = 4; a <= line.size();) {
+				size_t b = line.find('\t', a); if (b == std::string::npos) b = line.size();
+				const std::string field = line.substr(a, b - a);
+				if (field.compare(0, 3, "SN:") == 0 && !has_name) { name = field.substr(3); has_name = !name.empty(); }
+				else if (field.compare(0, 3, "LN:") == 0 && !has_length) {
+					u64 v = 0; bool ok = field.size() > 3 && field.size() <= 3 + 18;
+					for (size_t x = 3; ok && x < field.size(); ++x) { ok = field[x] >= '0' && field[x] <= '9'; v = v * 10 + (u64) (field[x] - '0'); }
+					has_length = ok && v > 0;
+				}
+				a = b + 1;
+			}
+			if (!has_name || !has_length) fail("failed to read SAM header");
+			reference(name);
+		}
+		if (lf == std::string::npos) return text.size();
+		p = lf + 1;
+	}
+}
+
 void read_chimeric_alignments(const std::string& bam_path, refdata& ref, const ingest_options& opt, fragment_table& out, coverage_windows& coverage, ingest_stats& stats) {
 	const int T = std::min(255, std::max(1, opt.threads));
 	const bool trace = getenv("ARB_TRACE") != NULL;
 	double tr_last = now_s();
 	auto lap = [&](const char* what) { if (trace) { const double t = now_s(); fprintf(stderr, "[ingest] %-28s %.3f s\n", what, t - tr_last); tr_last = t; } };
-	bgzf_file bam; bam.open(bam_path, T);
+	const u64 chunk_target = getenv("ARB_CHUNK_BYTES") ? (u64) atoll(getenv("ARB_CHUNK_BYTES")) : 128ull << 20; // env: test hook (many small chunks)
+	bgzf_file bam; bam.map(bam_path);
+	const input_format format = detect_format(bam, T, chunk_target);
 	lap("open + block table");
 	stats.t_inflate = stats.t_parse = stats.t_finalize = 0;
 	arb_ctx* const ctx = opt.scan_ctx;
 	auto check = [&](int rc, const char* what) { if (rc != 0) fail(std::string(what) + ": " + arb_last_error(ctx)); };
 
-	// chunks of ~128 MiB of decompressed data, each a whole number of BGZF blocks; a record that straddles a chunk boundary stays on the device for the next one
-	const u64 chunk_target = getenv("ARB_CHUNK_BYTES") ? (u64) atoll(getenv("ARB_CHUNK_BYTES")) : 128ull << 20; // env: test hook (many small chunks)
+	// chunks of ~128 MiB of decompressed data, each a whole number of BGZF blocks (pieces of a plain SAM file); a record (or line) that straddles a chunk
+	// boundary stays on the device for the next one
 	std::vector<u16> tid_to_contig; std::vector<u8> interesting_contig, viral_contig;
 	// A chunk is inflated by the host while the device copies and scans the previous one.
 	struct chunk_t { column<u8> buf /* page-locked: copied to the device asynchronously */; u64 pos /* in the inflated stream */; u64 first; bool last; chunk_t(): pos(0), first(0), last(false) {} };
@@ -266,26 +341,35 @@ void read_chimeric_alignments(const std::string& bam_path, refdata& ref, const i
 		c.last = b0 >= bam.blocks.size(); c.first = 0;
 		t_inflate += now_s() - ti;
 	};
+	auto add_reference = [&](const std::string& target) { // the next reference of the header (BAM or @SQ)
+		const u16 id = ref.contig_id(remove_chr(target));
+		ref.original_names[id] = target;
+		tid_to_contig.push_back(id);
+	};
+	std::string sq_names; std::vector<u64> sq_off(1, 0); // SAM: the @SQ names, for the RNAME lookup on the device
 	if (bam.blocks.empty()) fail("failed to read SAM header");
-	prepare(chunks[0]);
-	{ // the header: contig ids of the BAM's references
+	if (format != INPUT_BAM) {
+		const u64 header_end = read_sam_header(bam, [&](const std::string& name) { add_reference(name); sq_names += name; sq_off.push_back(sq_names.size()); });
+		while (b0 < bam.blocks.size() && bam.blocks[b0].out_off + bam.blocks[b0].out_len <= header_end) ++b0; // the first chunk starts at the block of the first record
+		prepare(chunks[0]);
+		chunks[0].first = header_end - chunks[0].pos;
+	} else { // the BAM header: contig ids of the BAM's references
+		prepare(chunks[0]);
 		const column<u8>& buf = chunks[0].buf;
 		if (buf.size() < 12 || memcmp(buf.data(), "BAM\1", 4) != 0) fail("failed to read SAM header");
 		const u32 l_text = rd32(buf.data() + 4);
 		if (12ull + l_text > buf.size()) fail("failed to read SAM header (header larger than one chunk)");
 		size_t p = 8 + l_text;
 		const u32 n_ref = rd32(buf.data() + p); p += 4;
-		tid_to_contig.resize(n_ref);
 		for (u32 k = 0; k < n_ref; ++k) {
 			if (p + 4 > buf.size()) fail("failed to read SAM header");
 			const u32 l_name = rd32(buf.data() + p); p += 4;
 			if (p + l_name + 4 > buf.size()) fail("failed to read SAM header");
-			const std::string target((const char*) buf.data() + p, strnlen((const char*) buf.data() + p, l_name)); p += l_name + 4;
-			const std::string name = remove_chr(target);
-			const u16 id = ref.contig_id(name);
-			ref.original_names[id] = target;
-			tid_to_contig[k] = id;
+			add_reference(std::string((const char*) buf.data() + p, strnlen((const char*) buf.data() + p, l_name))); p += l_name + 4;
 		}
+		chunks[0].first = p;
+	}
+	{ // the contig flags of the grown contig table, and the coverage windows
 		const size_t nc = ref.contig_ids.size();
 		interesting_contig.assign(nc, 0); viral_contig.assign(nc, 0);
 		for (std::map<std::string, u16>::iterator c = ref.contig_ids.begin(); c != ref.contig_ids.end(); ++c) {
@@ -295,7 +379,6 @@ void read_chimeric_alignments(const std::string& bam_path, refdata& ref, const i
 		}
 		ref.flatten(); // contig table may have grown
 		coverage.resize(ref);
-		chunks[0].first = p;
 	}
 	if (opt.after_header) opt.after_header(); // the grown contig table and the gene index go to the device
 	const u32 nc = (u32) ref.contig_ids.size();
@@ -304,6 +387,7 @@ void read_chimeric_alignments(const std::string& bam_path, refdata& ref, const i
 		for (u32 c = 0; c < nc; ++c) n_windows[c] = coverage.coverage[c].size();
 		check(arb_records_begin(ctx, tid_to_contig.data(), (u32) tid_to_contig.size(), interesting_contig.data(), viral_contig.data(), n_windows.data(), nc,
 		                        opt.max_itd_length, opt.external_duplicate_marking ? 1 : 0, bam.total_out), "arb_records_begin");
+		if (format != INPUT_BAM) check(arb_records_text_names(ctx, sq_names.data(), sq_off.data(), (u32) tid_to_contig.size()), "arb_records_text_names");
 	}
 	lap("header");
 	const u64 NO_ERROR = ~(u64) 0;
@@ -314,10 +398,11 @@ void read_chimeric_alignments(const std::string& bam_path, refdata& ref, const i
 		if (!c.last) next = std::thread([&]() { try { prepare(chunks[cur ^ 1]); } catch (const std::exception& x) { prepare_error = x.what(); if (prepare_error.empty()) prepare_error = "failed to load alignments"; } });
 		const double tp = now_s();
 		uint64_t n_records = 0, carry = 0, error = NO_ERROR; uint32_t malformed = 0;
-		const int rc = arb_records_chunk(ctx, c.buf.data(), c.buf.size(), c.first, c.pos, &n_records, &carry, &malformed, &error);
+		const int rc = format == INPUT_BAM ? arb_records_chunk(ctx, c.buf.data(), c.buf.size(), c.first, c.pos, &n_records, &carry, &malformed, &error)
+		                                   : arb_records_text_chunk(ctx, c.buf.data(), c.buf.size(), c.first, c.pos, c.last ? 1 : 0, &n_records, &carry, &error);
 		stats.t_parse += now_s() - tp;
 		if (next.joinable()) next.join();
-		check(rc, "arb_records_chunk");
+		check(rc, format == INPUT_BAM ? "arb_records_chunk" : "arb_records_text_chunk");
 		if (malformed) fail("failed to load alignments");
 		total_records += n_records;
 		if (error != NO_ERROR) { record_error = error; break; } // the replay may still find an earlier one (read-through fragments)

@@ -58,14 +58,12 @@ void engine::records_begin(const u16* tid_to_contig, u32 n_tid, const u8* intere
 	const char* bits = getenv("ARB_KEY_HASH_BITS");
 	rec_hash_mask = bits && atoi(bits) > 0 && atoi(bits) < 64 ? ((u64) 1 << atoi(bits)) - 1 : ~(u64) 0;
 	timings.bam_scan_ms = 0; timings.h2d_ms = 0; timings.h2d_bytes = 0;
-	timings.rec_chunk_copy_ms = timings.rec_chunk_kernels_ms = timings.rec_sort_ms = timings.rec_count_ms = timings.rec_scan_ms = timings.rec_write_ms = timings.rec_download_ms = 0;
+	timings.rec_chunk_copy_ms = timings.rec_chunk_kernels_ms = timings.rec_sort_ms = timings.rec_count_ms = timings.rec_scan_ms = timings.rec_write_ms = timings.rec_download_ms = timings.rec_text_parse_ms = 0;
 	rec_open = true;
 }
 
-void engine::records_chunk(const u8* chunk, u64 bytes, u64 first, u64 chunk_pos, u64* n_records, u64* carry, u32* malformed, u64* error) {
-	if (!rec_open) throw arb_error("arb_records_chunk without arb_records_begin");
-	stage_timer t_all(ex), t_copy(ex);
-	// the unfinished record at the end of the previous chunk goes in front of this one
+// the chunk goes to the device behind the unfinished record (or line) at the end of the previous one; returns the bytes of bam_buf now in use
+u64 engine::records_upload(const u8* chunk, u64 bytes) {
 	const u64 total = rec_carry + bytes;
 	if (total >= 0xFFFFFFF0ull) throw arb_error("failed to load alignments (chunk too large)");
 	bam_buf_next.ensure(total + 64);
@@ -78,18 +76,34 @@ void engine::records_chunk(const u8* chunk, u64 bytes, u64 first, u64 chunk_pos,
 	}
 	bam_buf_next.upload_at(ex, chunk, bytes, rec_carry);
 	bam_buf.swap(bam_buf_next);
+	return total;
+}
+
+void engine::records_chunk(const u8* chunk, u64 bytes, u64 first, u64 chunk_pos, u64* n_records, u64* carry, u32* malformed, u64* error) {
+	if (!rec_open) throw arb_error("arb_records_chunk without arb_records_begin");
+	stage_timer t_all(ex), t_copy(ex);
+	const u64 first_record = rec_carry ? 0 : first;
+	const u64 total = records_upload(chunk, bytes);
 	timings.rec_chunk_copy_ms += t_copy.stop();
 	stage_timer t_kernels(ex);
-	const u64 buf_pos = chunk_pos - rec_carry;
+	const u64 buf_pos = chunk_pos - (total - bytes);
 	u64 consumed = 0; u32 R = 0;
 	dbuf<u32> rec_off;
-	bam_scan(bam_buf.ptr(), total, rec_carry ? 0 : first, (i32) rec_n_tid, rec_off, &consumed, &R, malformed);
+	bam_scan(bam_buf.ptr(), total, first_record, (i32) rec_n_tid, rec_off, &consumed, &R, malformed);
 	*n_records = R;
 	rec_carry_at = consumed; rec_carry = total - consumed; *carry = rec_carry;
 	if (*malformed || R == 0) { rec_error.download(ex, error, 1); timings.rec_chunk_kernels_ms += t_kernels.stop(); timings.bam_scan_ms += t_all.stop(); return; }
+	records_store(bam_buf, buf_pos, total, rec_off.ptr(), R, chunk_pos + bytes, error);
+	timings.rec_chunk_kernels_ms += t_kernels.stop();
+	timings.bam_scan_ms += t_all.stop();
+}
+
+// the R records of B (block_size at B[rec_off[i]]; B[0] is at position buf_pos of the record stream, `total` bytes of B in use): classified, and the kept
+// ones appended to the store. seen = the bytes of the input read so far (with expected_bytes it sizes the store after the first chunk).
+void engine::records_store(const dbuf<u8>& B, u64 buf_pos, u64 total, const u32* rec_off, u32 R, u64 seen, u64* error) {
 	// classify, then append the kept records to the store
 	dbuf<u32> bytes_of((size_t) R + 1), kept((size_t) R + 1); dbuf<u64> hash(R); dbuf<i64> hit(R); dbuf<u8> sa(R);
-	const rec_chunk_view cv = {bam_buf.ptr(), rec_off.ptr(), buf_pos, rec_tid.ptr(), (i32) rec_n_tid, annot.contig_len.ptr(), rec_interesting.ptr()};
+	const rec_chunk_view cv = {B.ptr(), rec_off, buf_pos, rec_tid.ptr(), (i32) rec_n_tid, annot.contig_len.ptr(), rec_interesting.ptr()};
 	rec_extract_fn xf = {cv, rec_hash_mask, bytes_of.ptr(), kept.ptr(), hash.ptr(), hit.ptr(), sa.ptr(), rec_counters.ptr(), rec_error.ptr()};
 	for_each(ex, R, xf);
 	exclusive_scan_u32(ex, bytes_of.ptr(), bytes_of.ptr(), R); exclusive_scan_u32(ex, kept.ptr(), kept.ptr(), R);
@@ -99,7 +113,7 @@ void engine::records_chunk(const u8* chunk, u64 bytes, u64 first, u64 chunk_pos,
 	if (need_bytes > rec_arena.size() || need_items > rec_at.size()) {
 		// sized once from the share of the file seen so far (the first chunk), grown by a quarter where that falls short
 		double factor = 1.25;
-		if (rec_n == 0 && chunk_pos + bytes < rec_expected_bytes) factor = 1.03 * (double) rec_expected_bytes / (double) (chunk_pos + bytes);
+		if (rec_n == 0 && seen < rec_expected_bytes) factor = 1.03 * (double) rec_expected_bytes / (double) seen;
 		const u64 want_bytes = (u64) ((double) need_bytes * factor) + 4096, want_items = (u64) ((double) need_items * factor) + 1024;
 		if (want_items >= 0xFFFFFFF0ull) throw arb_error("more than 2^32 BAM records");
 		try {
@@ -121,13 +135,11 @@ void engine::records_chunk(const u8* chunk, u64 bytes, u64 first, u64 chunk_pos,
 	if (*error != ~(u64) 0 && rec_error_record.empty()) {
 		const u64 at = *error >> 3;
 		if (at >= buf_pos && at + 4 <= buf_pos + total) {
-			u8 bs[4]; bam_buf.download(ex, bs, 4, at - buf_pos);
+			u8 bs[4]; B.download(ex, bs, 4, at - buf_pos);
 			const u64 n = std::min<u64>(rec_rd32(bs), buf_pos + total - (at + 4));
-			rec_error_record.resize(n); bam_buf.download(ex, rec_error_record.data(), n, at - buf_pos + 4);
+			rec_error_record.resize(n); B.download(ex, rec_error_record.data(), n, at - buf_pos + 4);
 		}
 	}
-	timings.rec_chunk_kernels_ms += t_kernels.stop();
-	timings.bam_scan_ms += t_all.stop();
 }
 
 struct rec_seg_flag_fn { const u32* order; const u32* lo; const u32* hi; u32* flag; ARB_HD void operator()(u32 k) const { flag[k] = k == 0 || lo[order[k]] != lo[order[k - 1]] || hi[order[k]] != hi[order[k - 1]]; } };

@@ -69,7 +69,8 @@ class Timings(C.Structure):
                 ("genomic_support_ms", C.c_float), ("blacklist_ms", C.c_float), ("known_fusions_ms", C.c_float), ("tags_ms", C.c_float),
                 ("tags_match_ms", C.c_float), ("tags_sort_ms", C.c_float), ("tags_pairs", C.c_uint64), ("protein_domains_ms", C.c_float),
                 ("rec_chunk_copy_ms", C.c_float), ("rec_chunk_kernels_ms", C.c_float), ("rec_sort_ms", C.c_float), ("rec_count_ms", C.c_float),
-                ("rec_scan_ms", C.c_float), ("rec_write_ms", C.c_float), ("rec_download_ms", C.c_float)]
+                ("rec_scan_ms", C.c_float), ("rec_write_ms", C.c_float), ("rec_download_ms", C.c_float),
+                ("rec_text_parse_ms", C.c_float)]
 
 
 _CTYPE = {np.dtype(np.uint8): C.c_uint8, np.dtype(np.uint16): C.c_uint16, np.dtype(np.uint32): C.c_uint32, np.dtype(np.int32): C.c_int32,
@@ -540,7 +541,9 @@ def _np_from(pointer, n, dtype):
 
 
 class Pipeline:
-    """One run of the hot path on files: the call a user of the library makes (the `arriba` CLI is a thin wrapper over it)."""
+    """One run of the hot path on files: the call a user of the library makes (the `arriba` CLI is a thin wrapper over it).
+
+    `bam` is the alignment file: BAM, or SAM text (plain or BGZF-compressed), told apart by the content (DESIGN.md section 5)."""
 
     def __init__(self, bam, gtf, fasta, threads=1, device=0, lib_path=None, strandedness=3, params=None, output=None, discarded=None,
                  genomic_breakpoints=None, max_genomic_breakpoint_distance=100000, blacklist=None, known_fusions=None, tags=None, protein_domains=None):

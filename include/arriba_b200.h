@@ -141,6 +141,15 @@ int arb_records_begin(arb_ctx* ctx, const uint16_t* tid_to_contig, uint32_t n_ti
 int arb_records_chunk(arb_ctx* ctx, const uint8_t* chunk, uint64_t bytes, uint64_t first, uint64_t chunk_pos, uint64_t* n_records, uint64_t* carry, uint32_t* malformed, uint64_t* error);
 int arb_records_error_record(arb_ctx* ctx, const uint8_t** body, uint64_t* bytes);
 int arb_records_finish(arb_ctx* ctx, uint16_t* const* coverage, uint8_t* const* starts, uint8_t* const* ends, uint64_t* counters, uint64_t* error);
+/* SAM text input (DESIGN.md section 5 has the rules): after arb_records_begin, whose tid_to_contig maps the header's @SQ lines in file order,
+ *   arb_records_text_names : the @SQ names (name k = names[name_off[k], name_off[k + 1]), n_names = n_tid), which RNAME is looked up in,
+ *   arb_records_text_chunk : one chunk of the text stream (behind the @ header: first = the offset of the first record in the first chunk, else 0). The
+ *                            device cuts it into lines, stages every line as a BAM record body and classifies and stores those as arb_records_chunk does.
+ *                            The bytes after the last LF are kept for the next chunk (carry); with last != 0 they are the last line. error: as for
+ *                            arb_records_chunk, with positions in the stream of staged records, which keeps file order; an unreadable line is an error of
+ *                            kind 1. arb_records_error_record hands out the staged body. arb_records_finish follows as for BAM input. */
+int arb_records_text_names(arb_ctx* ctx, const char* names, const uint64_t* name_off, uint32_t n_names);
+int arb_records_text_chunk(arb_ctx* ctx, const uint8_t* chunk, uint64_t bytes, uint64_t first, uint64_t chunk_pos, int last, uint64_t* n_records, uint64_t* carry, uint64_t* error);
 int arb_fragment_table_build(arb_ctx* ctx, uint64_t sizes[6]);
 int arb_fragment_table_download(arb_ctx* ctx, const arb_soa_chunk* columns, char* names, uint64_t* name_off);
 /* ---- annotation of the resident fragments -------------------------------------------------------------------
@@ -431,6 +440,7 @@ typedef struct arb_timings {
 	float rec_scan_ms;          /* the exclusive scans of the tallies, the wrap count and the download of the totals */
 	float rec_write_ms;         /* the writing replay launches (pools and coverage counts) */
 	float rec_download_ms;      /* the coverage windows packed and brought back with the counters */
+	float rec_text_parse_ms;    /* SAM input, part of rec_chunk_kernels_ms: line ends, the parse and the staged BAM records, summed over the chunks */
 } arb_timings;
 int arb_get_timings(arb_ctx* ctx, arb_timings* out);
 /* Device scratch memory is pooled per device and survives arb_ctx_destroy so that the next sample reuses it; this returns it to the driver

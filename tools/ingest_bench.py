@@ -5,15 +5,19 @@ loaded outside the clock), a warm-up, then timed steps. One JSON line with the c
     writing launches, coverage and counter download of arb_records_finish,
   - finalize_rest_s: finalize less the device laps of arb_records_finish (the fragment-table build, its download and the host's share).
 Also the rate of a plain copy of one page-locked 128 MiB host buffer to the device in the same process: the PCIe floor of the chunk stream.
+With --sam (or --sam-bgzf) the SAM text rendering of the same world (tools/synth.cpp --sam-only, written once next to the BAM) is measured too: BAM and SAM
+steps alternate, after one warm-up of each, and every format gets its own medians, its input size and the SAM parse lap (rec_text_parse_ms, part of
+rec_chunk_kernels_ms).
 
-python tools/ingest_bench.py [--warmup 1] [--steps 3] [--threads N]"""
-import argparse, json, os, statistics, sys, time
+python tools/ingest_bench.py [--warmup 1] [--steps 3] [--threads N] [--sam | --sam-bgzf]"""
+import argparse, json, os, statistics, subprocess, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench
 from arriba_b200 import lib as L, _build
 
-LAPS = ["rec_chunk_copy_ms", "rec_chunk_kernels_ms", "rec_sort_ms", "rec_count_ms", "rec_scan_ms", "rec_write_ms", "rec_download_ms"]
+LAPS = ["rec_chunk_copy_ms", "rec_chunk_kernels_ms", "rec_sort_ms", "rec_count_ms", "rec_scan_ms", "rec_write_ms", "rec_download_ms", "rec_text_parse_ms"]
+FINISH_LAPS = ["rec_sort_ms", "rec_count_ms", "rec_scan_ms", "rec_write_ms", "rec_download_ms"]
 
 
 def pinned_h2d_gbps(reps=10):
@@ -29,15 +33,15 @@ def pinned_h2d_gbps(reps=10):
     return reps * (128 << 20) / (a.elapsed_time(b) * 1e-3) / 1e9
 
 
-def one_step(prefix, threads):
-    p = L.Pipeline(prefix + ".bam", prefix + ".gtf", prefix + ".fa", threads=threads)
+def one_step(prefix, threads, path=None):
+    p = L.Pipeline(path or prefix + ".bam", prefix + ".gtf", prefix + ".fa", threads=threads)
     p.step(L.STEP_LOAD_REFERENCE)
     t0 = time.perf_counter()
     p.step(L.STEP_INGEST)
     ingest_s = time.perf_counter() - t0
     s = p.stats(); t = p.context().timings()
     laps = {k: round(getattr(t, k), 2) for k in LAPS}
-    finish_ms = sum(laps[k] for k in LAPS[2:])
+    finish_ms = sum(laps[k] for k in FINISH_LAPS)
     r = {"ingest_s": round(ingest_s, 3), "ingest_split": {"inflate": round(s.t_inflate, 3), "parse": round(s.t_parse, 3), "finalize": round(s.t_finalize, 3)},
          "bam_scan_ms": round(t.bam_scan_ms, 1), "laps_ms": laps, "finalize_rest_s": round(s.t_finalize - finish_ms * 1e-3, 3),
          "records": int(s.n_records), "fragments": int(s.n_fragments)}
@@ -50,19 +54,37 @@ def main():
     ap.add_argument("--warmup", type=int, default=1); ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--threads", type=int, default=2 * (len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else 8))
     ap.add_argument("--workload", default="cfg2_10M_2x101_50k")
+    ap.add_argument("--sam", action="store_true", help="also the plain SAM rendering of the world")
+    ap.add_argument("--sam-bgzf", action="store_true", help="also the BGZF-compressed SAM rendering (level 1)")
     a = ap.parse_args()
     if not os.path.exists(_build.PRODUCT_LIB):
         _build.build_product()
     prefix = bench.ensure_world(a.workload)
     card = bench.ClockSampler(0).card()
+    inputs = {"bam": prefix + ".bam"}
+    if a.sam or a.sam_bgzf:
+        kind = "sam_bgzf" if a.sam_bgzf else "sam"
+        sam_prefix = prefix + "_" + kind
+        if not os.path.exists(sam_prefix + ".done"):
+            if not os.path.exists(sam_prefix + ".bam"):
+                os.symlink(prefix + ".bam", sam_prefix + ".bam")
+            subprocess.run([_build.build_tools(), "--prefix", sam_prefix, "--sam-only"] + (["--sam-bgzf", "1"] if a.sam_bgzf else []), check=True)
+            open(sam_prefix + ".done", "w").write("ok")
+        inputs[kind] = sam_prefix + ".sam"
     for _ in range(a.warmup):
-        one_step(prefix, a.threads)
-    steps = [one_step(prefix, a.threads) for _ in range(a.steps)]
-    med = lambda f: statistics.median(f(r) for r in steps)
-    out = {"workload": a.workload, "threads": a.threads, **card, "pinned_h2d_128MiB_GBps": round(pinned_h2d_gbps(), 2),
-           "median": {"ingest_s": med(lambda r: r["ingest_s"]), "finalize_s": med(lambda r: r["ingest_split"]["finalize"]), "bam_scan_ms": med(lambda r: r["bam_scan_ms"]),
-                      "laps_ms": {k: med(lambda r: r["laps_ms"][k]) for k in LAPS}},
-           "steps": steps}
+        for path in inputs.values():
+            one_step(prefix, a.threads, path)
+    steps = {k: [] for k in inputs}
+    for _ in range(a.steps):  # the formats alternate
+        for k, path in inputs.items():
+            steps[k].append(one_step(prefix, a.threads, path))
+    out = {"workload": a.workload, "threads": a.threads, **card, "pinned_h2d_128MiB_GBps": round(pinned_h2d_gbps(), 2)}
+    for k, st in steps.items():
+        med = lambda f: statistics.median(f(r) for r in st)
+        out[k] = {"input_bytes": os.path.getsize(inputs[k]),
+                  "median": {"ingest_s": med(lambda r: r["ingest_s"]), "finalize_s": med(lambda r: r["ingest_split"]["finalize"]), "bam_scan_ms": med(lambda r: r["bam_scan_ms"]),
+                             "laps_ms": {x: med(lambda r: r["laps_ms"][x]) for x in LAPS}},
+                  "steps": st}
     print(json.dumps(out))
 
 

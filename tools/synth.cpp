@@ -865,16 +865,68 @@ struct generator_t {
 	}
 };
 
+// ---------------------------------------------------------------------------------- the same records as SAM text (SAMv1 1.4), plain or BGZF
+static void write_sam(const string& bam_path, const string& sam_path, int bgzf_level /* < 0: plain text */) {
+	gzFile in = gzopen(bam_path.c_str(), "rb"); // reads every BGZF member
+	if (!in) { perror(bam_path.c_str()); exit(1); }
+	auto need = [&](void* p, unsigned n) { if (gzread(in, p, n) != (int) n) { fprintf(stderr, "synth: truncated BAM %s\n", bam_path.c_str()); exit(1); } };
+	auto rd32 = [&]() { uint32_t v; need(&v, 4); return v; };
+	char magic[4]; need(magic, 4);
+	string text(rd32(), '\0'); if (!text.empty()) need(&text[0], text.size());
+	vector<string> names(rd32());
+	for (size_t k = 0; k < names.size(); ++k) { string n(rd32(), '\0'); need(&n[0], n.size()); names[k] = n.c_str(); rd32(); }
+	FILE* plain = NULL; bam_writer_t z;
+	if (bgzf_level < 0) { plain = fopen(sam_path.c_str(), "wb"); if (!plain) { perror(sam_path.c_str()); exit(1); } } else z.open(sam_path, bgzf_level);
+	auto put = [&](const string& t) { if (plain) fwrite(t.data(), 1, t.size(), plain); else z.write(t.data(), t.size()); };
+	put(text.c_str());
+	static const char ops[] = "MIDNSHP=X", bases[] = "=ACMGRSVTWYHKDBN";
+	vector<unsigned char> b; string line;
+	uint32_t bs;
+	while (gzread(in, &bs, 4) == 4) {
+		b.resize(bs); need(b.data(), bs);
+		auto u32 = [&](size_t at) { uint32_t v; memcpy(&v, &b[at], 4); return v; };
+		auto u16 = [&](size_t at) { return (uint32_t) b[at] | (uint32_t) b[at + 1] << 8; };
+		const int32_t tid = (int32_t) u32(0), pos = (int32_t) u32(4), mtid = (int32_t) u32(20), mpos = (int32_t) u32(24), tlen = (int32_t) u32(28);
+		const uint32_t lq = b[8], mapq = b[9], nc = u16(12), flag = u16(14), ls = u32(16);
+		size_t at = 32;
+		line.assign((const char*) &b[at]); at += lq;
+		line += "\t" + to_string(flag) + "\t" + (tid < 0 ? string("*") : names[tid]) + "\t" + to_string(pos + 1) + "\t" + to_string(mapq) + "\t";
+		for (uint32_t k = 0; k < nc; ++k) { const uint32_t c = u32(at + 4 * k); line += to_string(c >> 4); line += ops[c & 15]; }
+		if (nc == 0) line += "*";
+		at += 4 * nc;
+		line += "\t" + (mtid < 0 ? string("*") : mtid == tid ? string("=") : names[mtid]) + "\t" + to_string(mpos + 1) + "\t" + to_string(tlen) + "\t";
+		for (uint32_t i = 0; i < ls; ++i) line += bases[(b[at + i / 2] >> (i & 1 ? 0 : 4)) & 15];
+		if (ls == 0) line += "*";
+		at += (ls + 1) / 2;
+		line += "\t";
+		for (uint32_t i = 0; i < ls; ++i) line += (char) (b[at + i] + 33);
+		if (ls == 0) line += "*";
+		at += ls;
+		while (at + 3 <= b.size()) { // the tags synth writes: C (integers) and Z
+			line += "\t"; line += (char) b[at]; line += (char) b[at + 1];
+			if (b[at + 2] == 'C') { line += ":i:" + to_string(b[at + 3]); at += 4; }
+			else { const string v((const char*) &b[at + 3]); line += ":Z:" + v; at += 3 + v.size() + 1; }
+		}
+		line += "\n";
+		put(line);
+	}
+	gzclose(in);
+	if (plain) fclose(plain); else z.close();
+}
+
 static void usage() {
 	fprintf(stderr,
 		"usage: synth --prefix P [--seed S] [--scale F] [--genes G] [--breakpoints B] [--fragments N] [--read-length L]\n"
 		"             [--normal-frac F] [--split-frac F] [--dup-frac F] [--multimap-frac F] [--mismapper-frac F] [--paralog-frac F]\n"
-		"             [--deep-frac F] [--deep-depth D] [--shuffle] [--varnames] [--compress LEVEL] [--chr] [--reads-only]\n");
+		"             [--deep-frac F] [--deep-depth D] [--shuffle] [--varnames] [--compress LEVEL] [--chr] [--reads-only]\n"
+		"             [--sam] [--sam-bgzf LEVEL] [--sam-only]\n"
+		"  --sam: also write P.sam, the records of P.bam as SAM text (--sam-bgzf: BGZF-compressed at LEVEL); --sam-only: convert an existing P.bam\n");
 	exit(1);
 }
 
 int main(int argc, char** argv) {
 	params_t P;
+	bool sam = false, sam_only = false; int sam_level = -1;
 	for (int i = 1; i < argc; ++i) {
 		string a = argv[i];
 		#define NEXT (i + 1 < argc ? argv[++i] : (usage(), (char*) NULL))
@@ -902,8 +954,12 @@ int main(int argc, char** argv) {
 		else if (a == "--chr") P.chr_prefix = true;
 		else if (a == "--reads-only") P.write_world = false;
 		else if (a == "--emit-breakpoints") P.emit_breakpoints = atoi(NEXT);
+		else if (a == "--sam") sam = true;
+		else if (a == "--sam-bgzf") { sam = true; sam_level = atoi(NEXT); }
+		else if (a == "--sam-only") { sam = true; sam_only = true; }
 		else usage();
 	}
+	if (sam_only) { write_sam(P.prefix + ".bam", P.prefix + ".sam", sam_level); return 0; }
 	rng_t rng(P.seed);
 	world_t w;
 	make_genome(w, P, rng);
@@ -915,6 +971,7 @@ int main(int argc, char** argv) {
 	}
 	generator_t gen(w, P);
 	gen.run(P.prefix + ".bam");
+	if (sam) write_sam(P.prefix + ".bam", P.prefix + ".sam", sam_level);
 	size_t total = 0; for (size_t c = 0; c < w.seq.size(); ++c) total += w.seq[c].size();
 	fprintf(stderr, "synth: genome=%zu bp, genes=%zu, breakpoints=%zu, chimeric fragments=%ld\n", total, w.genes.size(), w.bps.size(), gen.n_emitted_fragments);
 	return 0;
