@@ -113,6 +113,10 @@ int arb_records_begin(arb_ctx* ctx, const uint16_t* tid_to_contig, uint32_t n_ti
 int arb_records_chunk(arb_ctx* ctx, const uint8_t* chunk, uint64_t bytes, uint64_t first, uint64_t chunk_pos, uint64_t* n_records, uint64_t* carry, uint32_t* malformed, uint64_t* error) {
 	ARB_API_BEGIN(ctx) u64 r = 0, c = 0, e = 0; ctx->e.records_chunk(chunk, bytes, first, chunk_pos, &r, &c, malformed, &e); *n_records = r; *carry = c; *error = e; ARB_API_END(ctx)
 }
+int arb_records_source(arb_ctx* ctx, int chimeric_file, const uint16_t* tid_to_contig, uint32_t n_tid, uint64_t* first_position) {
+	ARB_API_BEGIN(ctx) u64 f = 0; ctx->e.records_source(chimeric_file != 0, tid_to_contig, n_tid, &f); *first_position = f; ARB_API_END(ctx)
+}
+int arb_fragment_table_chimeric_file(arb_ctx* ctx, uint64_t counts[2]) { ARB_API_BEGIN(ctx) counts[0] = ctx->e.ft_chimeric[0]; counts[1] = ctx->e.ft_chimeric[1]; ARB_API_END(ctx) }
 int arb_records_text_names(arb_ctx* ctx, const char* names, const uint64_t* name_off, uint32_t n_names) {
 	ARB_API_BEGIN(ctx) std::vector<u64> off(name_off, name_off + n_names + 1); ctx->e.records_text_names(names, off.data(), n_names); ARB_API_END(ctx)
 }

@@ -119,6 +119,7 @@ public:
 	void fragment_table_download(const arb_soa_chunk& columns, char* names, u64* name_off);
 	dbuf<arb_pool_fragment> pool_frags; dbuf<arb_pool_alignment> pool_alns; dbuf<char> pool_names, frag_names; dbuf<u32> pool_cigars; dbuf<u8> pool_seqs;
 	dbuf<u64> pool_base, frag_name_off; u32 pool_workers; u64 frag_name_bytes;
+	u64 ft_chimeric[2] = {0, 0}; // fragments of a separate chimeric file that the first malformed pass rejects / keeps (the last replay's counting pass)
 	// one sample on several GPUs (exchange.cu): replicated state travels as groups of device buffers, the work of find_fusions / filter_mismappers is divided
 	void exchange_header(int group, std::vector<u64>& header); void exchange_prepare(int group, const u64* header, u32 n_words);
 	void exchange_buffers(int group, std::vector<exchange_buffer>& out); void exchange_commit(int group);
@@ -160,6 +161,10 @@ public:
 	dbuf<u32> rec_hash_lo, rec_hash_hi, rec_cov_words, rec_cov_n; dbuf<u16> rec_tid;
 	u64 rec_n, rec_arena_used, rec_carry, rec_carry_at, rec_expected_bytes, rec_cov_windows, rec_hash_mask; u32 rec_n_tid, rec_n_contigs, rec_max_itd; bool rec_external_dup, rec_open;
 	std::vector<u8> rec_error_record; // the body of the record a chunk's error names
+	// a separate chimeric file (-c) ahead of the main file: the file whose chunks follow, its references; positions of later files start behind it
+	void records_source(bool chimeric_file, const u16* tid_to_contig, u32 n_tid, u64* first_position);
+	bool rec_src_chimeric = false /* the chunks are the -c file's */, rec_has_chimeric = false /* a -c file was selected since arb_records_begin */;
+	u64 rec_pos_base = 0 /* added to the positions of the current file */, rec_pos_end = 0 /* behind every position so far */, rec_chimeric_end = 0 /* positions below: -c records */;
 	// rows of the discarded-fusions file (rows.cu)
 	void set_row_texts(const arb_row_texts& t); void format_discarded_rows(const u8* confidence, u64* n_rows, u64* n_bytes); void get_row_text(char* out);
 	dbuf<char> row_gene_name, row_gene_id, row_contig_name, row_filter_name, row_text; dbuf<u32> row_gene_name_off, row_gene_id_off, row_contig_name_off, row_filter_name_off; dbuf<i32> row_exon_prev, row_exon_next;

@@ -23,10 +23,11 @@ struct ft_pools {
 	ARB_HD const char* name(u32 g, u32& len) const { const u32 w = worker_of(g); const arb_pool_fragment& f = frags[g]; len = f.name_len; return names + at(FT_NAMES, w) + f.name_off; }
 };
 
-// one alignment during normalisation: its fields, and its CIGAR as the pool's operations with at most four of them rewritten
-// (normalisation only touches the first two and the last two operations)
-struct ft_slot {
-	u16 contig; u8 supplementary, first_in_pair, forward; i32 start, end; u32 seq_len, cnt; u64 seq_off; const u32* ops;
+// one alignment during normalisation: its fields, and its CIGAR as the source's operations with at most four of them rewritten
+// (normalisation only touches the first two and the last two operations). OPS: where the operations come from -- the pool (const u32*), or a record of
+// the record store (records_hd.h), whose CIGAR need not be 4-byte aligned.
+template <class OPS> struct ft_slot_t {
+	u16 contig; u8 supplementary, first_in_pair, forward; i32 start, end; u32 seq_len, cnt; u64 seq_off; OPS ops;
 	u32 n_set, set_at[4], set_to[4];
 	// fixed trip counts: the arrays stay in registers
 	ARB_HD u32 op(u32 k) const {
@@ -45,9 +46,10 @@ struct ft_slot {
 	ARB_HD u32 back() const { return op(cnt - 1); }
 	ARB_HD u32 clip(bool at_front) const { const u32 c = at_front ? front() : back(), o = c & 15; return (o == C_S || o == C_H) ? c >> 4 : 0; }
 };
-ARB_HD void ft_swap(ft_slot& a, ft_slot& b) { const ft_slot t = a; a = b; b = t; }
+typedef ft_slot_t<const u32*> ft_slot;
+template <class S> ARB_HD void ft_swap(S& a, S& b) { const S t = a; a = b; b = t; }
 
-ARB_HD bool ft_disjoin(ft_slot& split, ft_slot& supp) {
+template <class S> ARB_HD bool ft_disjoin(S& split, S& supp) {
 	const u32 clipped_split = split.forward ? split.clip(true) : split.clip(false);
 	const u32 clipped_supp = supp.forward ? supp.clip(false) : supp.clip(true);
 	const int overlap = (int) split.seq_len - (int) clipped_split - (int) clipped_supp;
@@ -62,23 +64,14 @@ ARB_HD bool ft_disjoin(ft_slot& split, ft_slot& supp) {
 	return true;
 }
 
-// the slots of fragment g (0 = rejected), in the order MATE1, MATE2 / SPLIT_READ, SUPPLEMENTARY
-ARB_HD u32 ft_normalise(const ft_pools& p, u32 g, ft_slot (&m)[3]) {
-	const arb_pool_fragment& f = p.frags[g];
-	const bool single_end = f.single_end != 0;
-	if (single_end ? f.count != 2 : (f.count != 2 && f.count != 3)) return 0;
-	const u32 w = p.worker_of(g);
-	const u64 aln0 = p.at(FT_ALNS, w), cig0 = p.at(FT_CIGARS, w), seq0 = p.at(FT_SEQS, w);
-	i32 a = f.head;
-#pragma unroll
-	for (u32 s = 0; s < 3; ++s) {
-		if (s >= f.count) break;
-		const arb_pool_alignment& x = p.alns[aln0 + (u32) a];
-		m[s].contig = x.contig; m[s].supplementary = x.supplementary; m[s].first_in_pair = x.first_in_pair; m[s].forward = x.forward;
-		m[s].start = x.start; m[s].end = x.end; m[s].seq_len = x.seq_len; m[s].seq_off = seq0 + x.seq_off; m[s].cnt = x.cigar_cnt; m[s].ops = p.cigars + cig0 + x.cigar_off;
-		m[s].n_set = 0;
-		a = x.next;
-	}
+// the fragment sizes remove_malformed_alignments accepts at all
+ARB_HD bool ft_count_ok(bool single_end, u32 count) { return single_end ? count == 2 : (count == 2 || count == 3); }
+
+// The rule itself, on the fragment's alignments m[0, count) in the order the loop added them: brings them into the slots MATE1, MATE2 / SPLIT_READ,
+// SUPPLEMENTARY and returns how many it keeps, 0 = rejected. The fragment table applies it to the pools (ft_normalise); the record replay applies it to the
+// alignments that a separate chimeric file gave a read (records_hd.h), to learn whether the first pass over the map keeps them.
+template <class S> ARB_HD u32 ft_decide(bool single_end, u32 count, S (&m)[3]) {
+	if (!ft_count_ok(single_end, count)) return 0;
 	if (single_end) {
 		if (m[0].supplementary == m[1].supplementary) return 0;
 		// the longer anchor becomes the split read; it is duplicated into the MATE1 slot to imitate paired-end data
@@ -106,7 +99,7 @@ ARB_HD u32 ft_normalise(const ft_pools& p, u32 g, ft_slot (&m)[3]) {
 		if (flip) m[0].forward = !m[0].forward; else { m[1].forward = !m[1].forward; m[2].forward = !m[2].forward; }
 		m[0].first_in_pair = !flip; m[1].first_in_pair = flip; m[2].first_in_pair = flip;
 		if (!ft_disjoin(m[1], m[2])) return 0;
-	} else if (f.count == 3) {
+	} else if (count == 3) {
 		if (m[0].supplementary) ft_swap(m[0], m[2]); else if (m[1].supplementary) ft_swap(m[1], m[2]);
 		if (m[1].first_in_pair != m[2].first_in_pair) ft_swap(m[0], m[1]);
 		if (m[0].supplementary || m[1].supplementary || !m[2].supplementary) return 0;
@@ -116,16 +109,42 @@ ARB_HD u32 ft_normalise(const ft_pools& p, u32 g, ft_slot (&m)[3]) {
 		if (m[0].supplementary || m[1].supplementary) return 0;
 	}
 	for (int s = 0; s < 2; ++s) if ((m[s].front() & 15) == C_H || (m[s].back() & 15) == C_H) return 0; // anchors need their full sequence
-	return single_end ? 3 : f.count;
+	return single_end ? 3 : count;
+}
+
+// the slots of fragment g of the pools (0 = rejected), in the order MATE1, MATE2 / SPLIT_READ, SUPPLEMENTARY
+ARB_HD u32 ft_normalise(const ft_pools& p, u32 g, ft_slot (&m)[3]) {
+	const arb_pool_fragment& f = p.frags[g];
+	const bool single_end = f.single_end != 0;
+	if (!ft_count_ok(single_end, f.count)) return 0;
+	const u32 w = p.worker_of(g);
+	const u64 aln0 = p.at(FT_ALNS, w), cig0 = p.at(FT_CIGARS, w), seq0 = p.at(FT_SEQS, w);
+	i32 a = f.head;
+#pragma unroll
+	for (u32 s = 0; s < 3; ++s) {
+		if (s >= f.count) break;
+		const arb_pool_alignment& x = p.alns[aln0 + (u32) a];
+		m[s].contig = x.contig; m[s].supplementary = x.supplementary; m[s].first_in_pair = x.first_in_pair; m[s].forward = x.forward;
+		m[s].start = x.start; m[s].end = x.end; m[s].seq_len = x.seq_len; m[s].seq_off = seq0 + x.seq_off; m[s].cnt = x.cigar_cnt; m[s].ops = p.cigars + cig0 + x.cigar_off;
+		m[s].n_set = 0;
+		a = x.next;
+	}
+	return ft_decide(single_end, f.count, m);
 }
 
 ARB_HD u32 ft_seq_units(u32 seq_len) { return ((seq_len + 1) / 2 + 15) / 16; }
 
-struct ft_keep_fn { // per fragment of the pools: keep[g] (0/1), its CIGAR operations, sequence units and name length (0 for a rejected one); the longest kept name
+// per fragment of the pools: keep[g] (0/1), its CIGAR operations, sequence units and name length (0 for a rejected one); the longest kept name.
+// Fragments of a separate chimeric file (Chimeric.out.sam) went through remove_malformed_alignments twice in the reference: once after their own file
+// (the replay's counting pass counts that pass's verdicts) and once more with the main file's. The second pass keeps what the first kept, except single-end
+// fragments: the first pass made three alignments of their two and left them single-end, which the second pass rejects.
+struct ft_keep_fn {
 	ft_pools p; u32 *keep, *n_ops, *n_units, *name_len, *max_name_len;
 	ARB_HD void operator()(u32 g) const {
 		ft_slot m[3];
-		const u32 n = ft_normalise(p, g, m);
+		u32 n = ft_normalise(p, g, m);
+		const arb_pool_fragment& f = p.frags[g];
+		if (f.chimeric_file && f.single_end) n = 0;
 		u32 ops = 0, units = 0;
 #pragma unroll
 		for (u32 s = 0; s < 3; ++s) if (s < n) { ops += m[s].cnt; if (s < 2) units += ft_seq_units(m[s].seq_len); }

@@ -1,6 +1,6 @@
 // cli_main.cpp -- the `arriba` command line of arriba-b200: same option letters, defaults and error texts as the reference
 // (options.cpp:270-485, usage options.cpp:109-268), driving the pipeline through the public C ABI only.
-// Not supported (fail loudly): -c Chimeric.out.sam, -G, -I.
+// Not supported (fail loudly): -G, -I.
 #include <getopt.h>
 #include <unistd.h>
 #include <sys/resource.h>
@@ -35,8 +35,10 @@ static const char* FILTERS[] = {"", "duplicates", "inconsistently_clipped", "hom
 
 static void usage() {
 	std::cout << "arriba-b200: H100-native implementation of Arriba's post-alignment path (reference version 2.5.1 semantics)\n\n"
-	          << "Usage: arriba -x Aligned.out.bam -g annotation.gtf -a assembly.fa -o fusions.tsv [-O fusions.discarded.tsv] [OPTIONS]\n\n"
-	          << " -x FILE  BAM or SAM (plain or BGZF) with main and chimeric alignments (STAR --chimOutType WithinBAM)\n -g FILE  gene annotation (GTF)\n -a FILE  assembly (FastA)\n"
+	          << "Usage: arriba [-c Chimeric.out.sam] -x Aligned.out.bam -g annotation.gtf -a assembly.fa -o fusions.tsv [-O fusions.discarded.tsv] [OPTIONS]\n\n"
+	          << " -x FILE  BAM or SAM (plain or BGZF) with main and chimeric alignments (STAR --chimOutType WithinBAM)\n"
+	          << " -c FILE  chimeric alignments in a separate file (STAR --chimOutType SeparateSAMold: Chimeric.out.sam; SAM, BGZF SAM or BAM), read before -x\n"
+	          << " -g FILE  gene annotation (GTF)\n -a FILE  assembly (FastA)\n"
 	          << " -o FILE  output file   -O FILE  discarded candidates\n -f LIST  disable filters (comma/space separated)\n -s MODE  strandedness auto|yes|no|reverse\n"
 	          << " -i/-v contig lists, -E e-value cutoff, -S min support, -m/-L/-H/-R/-A/-M/-K/-V/-F/-U/-Q/-e/-l/-z/-Z thresholds as in the reference\n"
 	          << " -b FILE  blacklist (optionally .gz; required unless '-f blacklist')\n"
@@ -53,7 +55,7 @@ int main(int argc, char** argv) {
 	o.echo_progress = 1;
 	o.threads = (int) std::max(1u, std::min(32u, std::thread::hardware_concurrency()));
 	crash(argc > 1 && (std::string(argv[1]).empty() || argv[1][0] != '-'), std::string("cannot interpret the first argument: ") + argv[1]);
-	std::string bam, gtf, fasta, out, discarded, interesting, viral, blacklist, genomic, known_fusions, tags, protein_domains;
+	std::string bam, gtf, fasta, out, discarded, interesting, viral, blacklist, genomic, known_fusions, tags, protein_domains, chimeric;
 	opterr = 0;
 	const std::string valid = "c:x:d:g:G:o:O:t:p:a:b:k:s:i:v:f:E:S:m:L:H:D:R:A:M:K:V:F:U:Q:e:T:C:l:z:Z:@:uXIh";
 	std::map<char, unsigned> seen; int c; long iv; bool threads_given = false;
@@ -72,7 +74,14 @@ int main(int argc, char** argv) {
 			case 'k': known_fusions = optarg; crash(access(optarg, R_OK), "file not found/readable: " + known_fusions); break;
 			case 't': tags = optarg; crash(access(optarg, R_OK), "file not found/readable: " + tags); break;
 			case 'p': protein_domains = optarg; crash(access(optarg, R_OK), "file not found/readable: " + protein_domains); break;
-			case 'c': case 'G': case 'I':
+			case 'c': {
+				chimeric = optarg; crash(access(optarg, R_OK), "file not found/readable: " + chimeric);
+				const std::string junction_suffix = ".junction"; // options.cpp:280, 293-296
+				if (chimeric.size() >= junction_suffix.size() && chimeric.compare(chimeric.size() - junction_suffix.size(), junction_suffix.size(), junction_suffix) == 0)
+					std::cerr << "WARNING: it seems you passed the chimeric junction file ('Chimeric.out.junction') to the parameter -c, but this parameter takes the chimeric alignments file ('Chimeric.out.sam') as input" << std::endl;
+				break;
+			}
+			case 'G': case 'I':
 				crash(true, "option " + opt + " is not supported by arriba-b200 (see DESIGN.md, out of scope)"); break;
 			case 's': { const std::string m = optarg; o.strandedness = m == "auto" ? 3 : m == "yes" ? 1 : m == "no" ? 0 : m == "reverse" ? 2 : -1; crash(o.strandedness < 0, "invalid type of strandedness: " + m); break; }
 			case 'i': interesting = optarg; std::replace(interesting.begin(), interesting.end(), ',', ' '); break;
@@ -127,6 +136,7 @@ int main(int argc, char** argv) {
 	o.blacklist_file = blacklist.empty() ? NULL : blacklist.c_str();
 	o.known_fusions_file = known_fusions.empty() ? NULL : known_fusions.c_str(); o.tags_file = tags.empty() ? NULL : tags.c_str();
 	o.protein_domains_file = protein_domains.empty() ? NULL : protein_domains.c_str();
+	o.chimeric_file = chimeric.empty() ? NULL : chimeric.c_str();
 
 	arb_pipeline* p = NULL;
 	crash(arb_pipeline_create(&p, &o) != 0, arb_pipeline_error(NULL));

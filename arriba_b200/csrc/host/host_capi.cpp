@@ -29,7 +29,7 @@ void arb_default_run_options(arb_run_options* o) {
 	o->min_support = 2; o->min_anchor_length = 23; o->min_spliced_events = 4; o->high_expression_quantile = 0.998f; o->exonic_fraction = 0.33f;
 	o->min_itd_allele_fraction = 0.07f; o->min_itd_support = 10; o->print_extra_info_for_discarded_fusions = 0; o->echo_progress = 0;
 	o->top_viral_contigs = 5; o->viral_contig_min_covered_fraction = 0.05f;
-	o->genomic_breakpoints_file = NULL; o->max_genomic_breakpoint_distance = 100000; o->blacklist_file = NULL; o->known_fusions_file = NULL; o->tags_file = NULL; o->protein_domains_file = NULL;
+	o->genomic_breakpoints_file = NULL; o->max_genomic_breakpoint_distance = 100000; o->blacklist_file = NULL; o->known_fusions_file = NULL; o->tags_file = NULL; o->protein_domains_file = NULL; o->chimeric_file = NULL;
 }
 
 // Dozens of host threads allocate and free at the same time (record parsing, annotation, row formatting). glibc gives every thread its own arena, but arenas
@@ -66,6 +66,7 @@ int arb_pipeline_create(arb_pipeline** out, const arb_run_options* o) {
 		if (o->known_fusions_file) r.known_fusions_file = o->known_fusions_file;
 		if (o->tags_file) r.tags_file = o->tags_file;
 		if (o->protein_domains_file) r.protein_domains_file = o->protein_domains_file;
+		if (o->chimeric_file) r.chimeric_file = o->chimeric_file;
 		r.params = o->params; r.strandedness = o->strandedness; r.fragment_length = o->fragment_length; r.threads = o->threads; r.device = o->device;
 		*out = x;
 	} catch (const std::exception& e) { g_pipeline_create_error = e.what(); return 1; }
@@ -112,6 +113,7 @@ int arb_pipeline_stats(arb_pipeline* x, arb_run_stats* s) {
 	s->t_inflate = p.istats.t_inflate; s->t_parse = p.istats.t_parse; s->t_finalize = p.istats.t_finalize;
 	for (int q = 0; q < 32 && q < EV_COUNT; ++q) s->event_seconds[q] = p.t_events[q];
 	s->output_seconds = p.t_output; s->n_candidates = p.ev.n;
+	s->chimeric_records = p.istats.chimeric_records; s->chimeric_malformed = p.istats.chimeric_malformed; s->chimeric_total = p.istats.chimeric_total;
 	for (arb::u32 q = 0; q < p.ev.n; ++q) if (p.ev.filter[q] == 0) ++s->n_unfiltered_candidates;
 	const arb::host::fragment_table& f = p.frags;
 	s->h2d_bytes = f.n_aln.size() + f.fflags.size() + f.filter.size() + f.aflags.size() + 2 * (f.contig.size() + f.cigar_cnt.size() + f.seq_len.size() + f.genes_cnt.size()) +

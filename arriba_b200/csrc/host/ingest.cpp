@@ -224,20 +224,23 @@ frag_view fragment_table::view() {
 }
 
 
-// the text of a fatal record error (records_hd.h: kinds and order)
+// the text of a fatal record error (records_hd.h: kinds and order); tid_to_contig: the map of the file the record came from
 static std::string record_error_text(u64 error, arb_ctx* ctx, const std::vector<u16>& tid_to_contig, const refdata& ref) {
 	const u32 kind = (u32) (error & 7);
 	if (kind == REC_ERR_ANNOTATION) return "too many overlapping annotation records at one locus";
-	if (kind == REC_ERR_CIGAR || kind == REC_ERR_BEYOND) {
+	if (kind == REC_ERR_CIGAR || kind == REC_ERR_BEYOND || kind == REC_ERR_UNMAPPED) {
 		const uint8_t* body = NULL; uint64_t n = 0;
 		rec_t r;
-		if (arb_records_error_record(ctx, &body, &n) == 0 && body && rec_parse(body, (u32) n, r) && r.tid >= 0 && (size_t) r.tid < tid_to_contig.size()) {
+		if (arb_records_error_record(ctx, &body, &n) == 0 && body && rec_parse(body, (u32) n, r)) {
 			const std::string name(r.qname(), r.name_len());
-			const u32 contig = tid_to_contig[r.tid];
-			i64 query_span = 0;
-			rec_validate(r, ref.has_sequence(contig) ? (u32) ref.seq_len[contig] : 0, query_span);
-			if (kind == REC_ERR_CIGAR) return "CIGAR string of read '" + name + "' does not fit its sequence (" + std::to_string(query_span) + " bases in " + std::to_string(r.n_cigar) + " operations, sequence of " + std::to_string(r.l_seq) + ")";
-			return "alignment of read '" + name + "' extends beyond the end of contig '" + ref.original_names[contig] + "' (was the file aligned to another assembly?)";
+			if (kind == REC_ERR_UNMAPPED) return "alignment of read '" + name + "' in the chimeric alignment file has no reference sequence (the file must hold mapped records only, as STAR writes Chimeric.out.sam)";
+			if (r.tid >= 0 && (size_t) r.tid < tid_to_contig.size()) {
+				const u32 contig = tid_to_contig[r.tid];
+				i64 query_span = 0;
+				rec_validate(r, ref.has_sequence(contig) ? (u32) ref.seq_len[contig] : 0, query_span);
+				if (kind == REC_ERR_CIGAR) return "CIGAR string of read '" + name + "' does not fit its sequence (" + std::to_string(query_span) + " bases in " + std::to_string(r.n_cigar) + " operations, sequence of " + std::to_string(r.l_seq) + ")";
+				return "alignment of read '" + name + "' extends beyond the end of contig '" + ref.original_names[contig] + "' (was the file aligned to another assembly?)";
+			}
 		}
 	}
 	return "failed to load alignments";
@@ -306,68 +309,63 @@ template <class F> static u64 read_sam_header(const bgzf_file& f, F reference) {
 	}
 }
 
+// The BAM header (magic, text, references), however many blocks it spans; every reference's name goes to `reference`. Returns the offset of the first
+// record in the inflated stream.
+template <class F> static u64 read_bam_header(const bgzf_file& f, F reference) {
+	std::vector<u8> h; size_t inflated = 0;
+	auto have = [&](u64 n) { // the first n bytes of the stream are in h
+		if (n > f.total_out) return false;
+		while (h.size() < n && inflated < f.blocks.size()) { const size_t at = h.size(); h.resize(at + f.blocks[inflated].out_len); f.inflate_block(f.blocks[inflated], h.data() + at); ++inflated; }
+		return h.size() >= n;
+	};
+	if (!have(12) || memcmp(h.data(), "BAM\1", 4) != 0) fail("failed to read SAM header");
+	u64 p = 8ull + rd32(h.data() + 4);
+	if (!have(p + 4)) fail("failed to read SAM header");
+	const u32 n_ref = rd32(h.data() + p); p += 4;
+	for (u32 k = 0; k < n_ref; ++k) {
+		if (!have(p + 4)) fail("failed to read SAM header");
+		const u32 l_name = rd32(h.data() + p); p += 4;
+		if (!have(p + l_name + 4)) fail("failed to read SAM header");
+		reference(std::string((const char*) h.data() + p, strnlen((const char*) h.data() + p, l_name))); p += l_name + 4;
+	}
+	return p;
+}
+
+// one input file: its blocks, format and header (the contig id of every reference; SAM: the @SQ names, for the RNAME lookup on the device)
+struct input_file {
+	bgzf_file f; input_format format; u64 header_end; std::vector<u16> tid_to_contig; std::string sq_names; std::vector<u64> sq_off;
+	input_file(): format(INPUT_BAM), header_end(0), sq_off(1, 0) {}
+};
+
 void read_chimeric_alignments(const std::string& bam_path, refdata& ref, const ingest_options& opt, fragment_table& out, coverage_windows& coverage, ingest_stats& stats) {
 	const int T = std::min(255, std::max(1, opt.threads));
 	const bool trace = getenv("ARB_TRACE") != NULL;
 	double tr_last = now_s();
 	auto lap = [&](const char* what) { if (trace) { const double t = now_s(); fprintf(stderr, "[ingest] %-28s %.3f s\n", what, t - tr_last); tr_last = t; } };
 	const u64 chunk_target = getenv("ARB_CHUNK_BYTES") ? (u64) atoll(getenv("ARB_CHUNK_BYTES")) : 128ull << 20; // env: test hook (many small chunks)
-	bgzf_file bam; bam.map(bam_path);
-	const input_format format = detect_format(bam, T, chunk_target);
+	// A separate chimeric file (-c) is read first, in a call of its own in the reference (arriba.cpp:123-130): its header, then the main file's, name the
+	// contigs (ids in that order; a contig's printed name is the last header's spelling), its records go into the store ahead of the main file's.
+	const bool has_chimeric = !opt.chimeric_path.empty();
+	input_file chim, main_file;
+	if (has_chimeric) { chim.f.map(opt.chimeric_path); chim.format = detect_format(chim.f, T, chunk_target); }
+	main_file.f.map(bam_path); main_file.format = detect_format(main_file.f, T, chunk_target);
 	lap("open + block table");
 	stats.t_inflate = stats.t_parse = stats.t_finalize = 0;
+	stats.chimeric_records = stats.chimeric_malformed = stats.chimeric_total = 0;
 	arb_ctx* const ctx = opt.scan_ctx;
 	auto check = [&](int rc, const char* what) { if (rc != 0) fail(std::string(what) + ": " + arb_last_error(ctx)); };
 
-	// chunks of ~128 MiB of decompressed data, each a whole number of BGZF blocks (pieces of a plain SAM file); a record (or line) that straddles a chunk
-	// boundary stays on the device for the next one
-	std::vector<u16> tid_to_contig; std::vector<u8> interesting_contig, viral_contig;
-	// A chunk is inflated by the host while the device copies and scans the previous one.
-	struct chunk_t { column<u8> buf /* page-locked: copied to the device asynchronously */; u64 pos /* in the inflated stream */; u64 first; bool last; chunk_t(): pos(0), first(0), last(false) {} };
-	chunk_t chunks[2];
-	size_t b0 = 0;
-	double t_inflate = 0; // written by the inflating thread only
-	auto prepare = [&](chunk_t& c) {
-		const double ti = now_s();
-		size_t b1 = b0; u64 bytes = 0;
-		while (b1 < bam.blocks.size() && (bytes == 0 || bytes + bam.blocks[b1].out_len <= chunk_target)) bytes += bam.blocks[b1++].out_len;
-		column<u8>& buf = c.buf;
-		if (buf.capacity() < bytes) buf.reserve(bytes + (16u << 20)); // one page-locked block per buffer for the whole file (chunks differ a little in size)
-		buf.resize(bytes);
-		c.pos = b0 < bam.blocks.size() ? bam.blocks[b0].out_off : bam.total_out;
-		const size_t first = b0;
-		parallel_for(T, b1 - first, [&](int, size_t lo, size_t hi) { for (size_t b = first + lo; b < first + hi; ++b) bam.inflate_block(bam.blocks[b], buf.data() + (bam.blocks[b].out_off - c.pos)); });
-		b0 = b1;
-		c.last = b0 >= bam.blocks.size(); c.first = 0;
-		t_inflate += now_s() - ti;
-	};
-	auto add_reference = [&](const std::string& target) { // the next reference of the header (BAM or @SQ)
-		const u16 id = ref.contig_id(remove_chr(target));
-		ref.original_names[id] = target;
-		tid_to_contig.push_back(id);
-	};
-	std::string sq_names; std::vector<u64> sq_off(1, 0); // SAM: the @SQ names, for the RNAME lookup on the device
-	if (bam.blocks.empty()) fail("failed to read SAM header");
-	if (format != INPUT_BAM) {
-		const u64 header_end = read_sam_header(bam, [&](const std::string& name) { add_reference(name); sq_names += name; sq_off.push_back(sq_names.size()); });
-		while (b0 < bam.blocks.size() && bam.blocks[b0].out_off + bam.blocks[b0].out_len <= header_end) ++b0; // the first chunk starts at the block of the first record
-		prepare(chunks[0]);
-		chunks[0].first = header_end - chunks[0].pos;
-	} else { // the BAM header: contig ids of the BAM's references
-		prepare(chunks[0]);
-		const column<u8>& buf = chunks[0].buf;
-		if (buf.size() < 12 || memcmp(buf.data(), "BAM\1", 4) != 0) fail("failed to read SAM header");
-		const u32 l_text = rd32(buf.data() + 4);
-		if (12ull + l_text > buf.size()) fail("failed to read SAM header (header larger than one chunk)");
-		size_t p = 8 + l_text;
-		const u32 n_ref = rd32(buf.data() + p); p += 4;
-		for (u32 k = 0; k < n_ref; ++k) {
-			if (p + 4 > buf.size()) fail("failed to read SAM header");
-			const u32 l_name = rd32(buf.data() + p); p += 4;
-			if (p + l_name + 4 > buf.size()) fail("failed to read SAM header");
-			add_reference(std::string((const char*) buf.data() + p, strnlen((const char*) buf.data() + p, l_name))); p += l_name + 4;
-		}
-		chunks[0].first = p;
+	std::vector<u8> interesting_contig, viral_contig;
+	for (input_file* in : {&chim, &main_file}) {
+		if (in == &chim && !has_chimeric) continue;
+		if (in->f.blocks.empty()) fail("failed to read SAM header");
+		auto add_reference = [&](const std::string& target) { // the next reference of the header (BAM or @SQ)
+			const u16 id = ref.contig_id(remove_chr(target));
+			ref.original_names[id] = target;
+			in->tid_to_contig.push_back(id);
+		};
+		if (in->format != INPUT_BAM) in->header_end = read_sam_header(in->f, [&](const std::string& name) { add_reference(name); in->sq_names += name; in->sq_off.push_back(in->sq_names.size()); });
+		else in->header_end = read_bam_header(in->f, add_reference);
 	}
 	{ // the contig flags of the grown contig table, and the coverage windows
 		const size_t nc = ref.contig_ids.size();
@@ -385,30 +383,69 @@ void read_chimeric_alignments(const std::string& bam_path, refdata& ref, const i
 	{
 		std::vector<u64> n_windows(nc);
 		for (u32 c = 0; c < nc; ++c) n_windows[c] = coverage.coverage[c].size();
-		check(arb_records_begin(ctx, tid_to_contig.data(), (u32) tid_to_contig.size(), interesting_contig.data(), viral_contig.data(), n_windows.data(), nc,
-		                        opt.max_itd_length, opt.external_duplicate_marking ? 1 : 0, bam.total_out), "arb_records_begin");
-		if (format != INPUT_BAM) check(arb_records_text_names(ctx, sq_names.data(), sq_off.data(), (u32) tid_to_contig.size()), "arb_records_text_names");
+		check(arb_records_begin(ctx, main_file.tid_to_contig.data(), (u32) main_file.tid_to_contig.size(), interesting_contig.data(), viral_contig.data(), n_windows.data(), nc,
+		                        opt.max_itd_length, opt.external_duplicate_marking ? 1 : 0, main_file.f.total_out + (has_chimeric ? chim.f.total_out : 0)), "arb_records_begin");
 	}
 	lap("header");
+
+	// chunks of ~128 MiB of decompressed data, each a whole number of BGZF blocks (pieces of a plain SAM file); a record (or line) that straddles a chunk
+	// boundary stays on the device for the next one
+	// A chunk is inflated by the host while the device copies and scans the previous one.
+	struct chunk_t { column<u8> buf /* page-locked: copied to the device asynchronously */; u64 pos /* in the inflated stream */; u64 first; bool last; chunk_t(): pos(0), first(0), last(false) {} };
+	chunk_t chunks[2];
+	double t_inflate = 0; // written by the inflating thread only
 	const u64 NO_ERROR = ~(u64) 0;
-	u64 total_records = 0, record_error = NO_ERROR;
-	for (int cur = 0;; cur ^= 1) {
-		chunk_t& c = chunks[cur];
-		std::string prepare_error; std::thread next;
-		if (!c.last) next = std::thread([&]() { try { prepare(chunks[cur ^ 1]); } catch (const std::exception& x) { prepare_error = x.what(); if (prepare_error.empty()) prepare_error = "failed to load alignments"; } });
-		const double tp = now_s();
-		uint64_t n_records = 0, carry = 0, error = NO_ERROR; uint32_t malformed = 0;
-		const int rc = format == INPUT_BAM ? arb_records_chunk(ctx, c.buf.data(), c.buf.size(), c.first, c.pos, &n_records, &carry, &malformed, &error)
-		                                   : arb_records_text_chunk(ctx, c.buf.data(), c.buf.size(), c.first, c.pos, c.last ? 1 : 0, &n_records, &carry, &error);
-		stats.t_parse += now_s() - tp;
-		if (next.joinable()) next.join();
-		check(rc, format == INPUT_BAM ? "arb_records_chunk" : "arb_records_text_chunk");
-		if (malformed) fail("failed to load alignments");
-		total_records += n_records;
-		if (error != NO_ERROR) { record_error = error; break; } // the replay may still find an earlier one (read-through fragments)
-		if (!prepare_error.empty()) fail(prepare_error);
-		if (c.last) { if (carry) fail("failed to load alignments"); break; } // truncated file
+	u64 record_error = NO_ERROR, main_first = 0;
+	// the records of one file; returns their number (record_error set: stopped at the chunk that has the error)
+	auto read_records = [&](input_file& in) {
+		const bgzf_file& bam = in.f;
+		size_t b0 = 0;
+		auto prepare = [&](chunk_t& c) {
+			const double ti = now_s();
+			size_t b1 = b0; u64 bytes = 0;
+			while (b1 < bam.blocks.size() && (bytes == 0 || bytes + bam.blocks[b1].out_len <= chunk_target)) bytes += bam.blocks[b1++].out_len;
+			column<u8>& buf = c.buf;
+			if (buf.capacity() < bytes) buf.reserve(bytes + (16u << 20)); // one page-locked block per buffer for the whole file (chunks differ a little in size)
+			buf.resize(bytes);
+			c.pos = b0 < bam.blocks.size() ? bam.blocks[b0].out_off : bam.total_out;
+			const size_t first = b0;
+			parallel_for(T, b1 - first, [&](int, size_t lo, size_t hi) { for (size_t b = first + lo; b < first + hi; ++b) bam.inflate_block(bam.blocks[b], buf.data() + (bam.blocks[b].out_off - c.pos)); });
+			b0 = b1;
+			c.last = b0 >= bam.blocks.size(); c.first = 0;
+			t_inflate += now_s() - ti;
+		};
+		while (b0 < bam.blocks.size() && bam.blocks[b0].out_off + bam.blocks[b0].out_len <= in.header_end) ++b0; // the first chunk starts at the block of the first record
+		prepare(chunks[0]);
+		chunks[0].first = in.header_end - chunks[0].pos;
+		if (in.format != INPUT_BAM) check(arb_records_text_names(ctx, in.sq_names.data(), in.sq_off.data(), (u32) in.tid_to_contig.size()), "arb_records_text_names");
+		u64 total_records = 0;
+		for (int cur = 0;; cur ^= 1) {
+			chunk_t& c = chunks[cur];
+			std::string prepare_error; std::thread next;
+			if (!c.last) next = std::thread([&]() { try { prepare(chunks[cur ^ 1]); } catch (const std::exception& x) { prepare_error = x.what(); if (prepare_error.empty()) prepare_error = "failed to load alignments"; } });
+			const double tp = now_s();
+			uint64_t n_records = 0, carry = 0, error = NO_ERROR; uint32_t malformed = 0;
+			const int rc = in.format == INPUT_BAM ? arb_records_chunk(ctx, c.buf.data(), c.buf.size(), c.first, c.pos, &n_records, &carry, &malformed, &error)
+			                                      : arb_records_text_chunk(ctx, c.buf.data(), c.buf.size(), c.first, c.pos, c.last ? 1 : 0, &n_records, &carry, &error);
+			stats.t_parse += now_s() - tp;
+			if (next.joinable()) next.join();
+			check(rc, in.format == INPUT_BAM ? "arb_records_chunk" : "arb_records_text_chunk");
+			if (malformed) fail("failed to load alignments");
+			total_records += n_records;
+			if (error != NO_ERROR) { record_error = error; break; } // the replay may still find an earlier one (read-through fragments)
+			if (!prepare_error.empty()) fail(prepare_error);
+			if (c.last) { if (carry) fail("failed to load alignments"); break; } // truncated file
+		}
+		return total_records;
+	};
+	if (has_chimeric) {
+		u64 first = 0;
+		check(arb_records_source(ctx, 1, chim.tid_to_contig.data(), (u32) chim.tid_to_contig.size(), &first), "arb_records_source");
+		stats.chimeric_records = read_records(chim);
+		if (record_error == NO_ERROR) check(arb_records_source(ctx, 0, main_file.tid_to_contig.data(), (u32) main_file.tid_to_contig.size(), &main_first), "arb_records_source");
+		else main_first = NO_ERROR; // the main file is not read
 	}
+	stats.records = record_error == NO_ERROR ? read_records(main_file) : 0;
 	if (trace) fprintf(stderr, "[ingest]   of which inflate %.3f s (overlaps with) chunk copies + record extraction %.3f s\n", t_inflate, stats.t_parse);
 	stats.t_inflate = t_inflate;
 	{ chunk_t a, b; std::swap(chunks[0], a); std::swap(chunks[1], b); }
@@ -424,21 +461,44 @@ void read_chimeric_alignments(const std::string& bam_path, refdata& ref, const i
 		check(arb_records_finish(ctx, cov.data(), starts.data(), ends.data(), (uint64_t*) counters.data(), &error), "arb_records_finish");
 		if (error != NO_ERROR) record_error = std::min<u64>(record_error, error);
 	}
-	if (record_error != NO_ERROR) fail(record_error_text(record_error, ctx, tid_to_contig, ref));
+	const char* no_chimeric_reads = "no split reads or discordant mates found (STAR must either be run with '--chimOutType WithinBAM' or the file 'Chimeric.out.sam' must be passed to Arriba via the argument -c)";
+	// The end of the -c file's call: its first malformed pass (the replay's counting pass has its verdicts, also when the main file has a record error), its
+	// warning, its lack of chimeric reads, its progress line. All of it comes before any error of the main file.
+	auto chimeric_file_done = [&]() {
+		uint64_t c[2];
+		check(arb_fragment_table_chimeric_file(ctx, c), "arb_fragment_table_chimeric_file");
+		stats.chimeric_malformed = c[0]; stats.chimeric_total = c[1];
+		if (c[0] > 0) std::cerr << "WARNING: " << c[0] << " SAM records were malformed and ignored" << std::endl;
+		if (counters[REC_CTR_CHIMERIC] == 0) fail(no_chimeric_reads);
+		if (opt.chimeric_done) opt.chimeric_done(c[1]);
+	};
+	if (record_error != NO_ERROR) {
+		const bool in_chimeric_file = has_chimeric && (record_error >> 3) < main_first;
+		if (has_chimeric && !in_chimeric_file) chimeric_file_done();
+		fail(record_error_text(record_error, ctx, in_chimeric_file ? chim.tid_to_contig : main_file.tid_to_contig, ref));
+	}
 	lap("replay (device)");
 	stats.mapped_reads = counters[REC_CTR_MAPPED]; stats.malformed = counters[REC_CTR_MALFORMED]; stats.missing_hi_tag = counters[REC_CTR_MISSING_HI];
-	stats.records = total_records; stats.no_chimeric_reads = counters[REC_CTR_CHIMERIC] == 0;
+	stats.no_chimeric_reads = counters[REC_CTR_CHIMERIC] == 0;
 	stats.mapped_viral_reads_by_contig.assign(counters.begin() + REC_CTR_VIRAL, counters.end());
-	if (stats.mapped_reads == 0) fail("no normal reads found");
+	if (!has_chimeric && stats.mapped_reads == 0) fail("no normal reads found");
 
 	// ---- the fragment table, built on the device from the pools (csrc/fragtable.cu): slot normalisation and rejection of
 	// malformed fragments (read_chimeric_alignments.cpp:340-506), name order, SoA columns, multimapper flags (:792-802) ----
 	uint64_t sizes[6];
 	check(arb_fragment_table_build(ctx, sizes), "arb_fragment_table_build");
 	lap("normalise + name order + columns (device)");
-	stats.malformed += sizes[1]; stats.multimapper_pairs = sizes[5];
-	if (stats.malformed > 0) std::cerr << "WARNING: " << stats.malformed << " SAM records were malformed and ignored" << std::endl;
-	if (stats.no_chimeric_reads) fail("no split reads or discordant mates found (STAR must either be run with '--chimOutType WithinBAM' or the file 'Chimeric.out.sam' must be passed to Arriba via the argument -c)");
+	stats.multimapper_pairs = sizes[5];
+	if (has_chimeric) { // the -c file's call ends, then the main file's
+		chimeric_file_done();
+		if (stats.mapped_reads == 0) fail("no normal reads found");
+		stats.malformed += sizes[1] - stats.chimeric_malformed;
+		if (stats.malformed > 0) std::cerr << "WARNING: " << stats.malformed << " SAM records were malformed and ignored" << std::endl;
+	} else {
+		stats.malformed += sizes[1];
+		if (stats.malformed > 0) std::cerr << "WARNING: " << stats.malformed << " SAM records were malformed and ignored" << std::endl;
+		if (stats.no_chimeric_reads) fail(no_chimeric_reads);
+	}
 	if (stats.missing_hi_tag > 0) std::cerr << "WARNING: " << stats.missing_hi_tag << " secondary alignments lack the 'HI' tag and were ignored (STAR must be run with '--outSAMattributes HI' for Arriba to make use of multi-mapping reads for fusion detection)" << std::endl;
 
 	// ---- the host's copy of the table (fragment length, strandedness, the mate swaps, the writer, the broadcast of a sharded run read it) ----

@@ -1,8 +1,8 @@
 // ingest.h -- chimeric BAM ingest: BGZF inflate on host threads, the record loop on the device, into structure-of-arrays fragment columns
 // (arb_soa_chunk layout, fragments in name order), plus the by-products the later stages need (mapped read count,
 // coverage windows). Behavioural contract: read_chimeric_alignments (read_chimeric_alignments.cpp:560-773) and helpers
-// (:19-558), mark_multimappers (:792-802), coverage_t (read_stats.cpp:148-306). Only STAR "WithinBAM" input (-x) is
-// handled; Chimeric.out.sam (-c), SAM text and CRAM are not.
+// (:19-558), mark_multimappers (:792-802), coverage_t (read_stats.cpp:148-306). Input: BAM or SAM text (-x), STAR "WithinBAM" or, with
+// STAR's Chimeric.out.sam (-c) read first, "SeparateSAMold"; CRAM is not read.
 #pragma once
 #include <string>
 #include <vector>
@@ -72,6 +72,7 @@ struct fragment_table { // host image of arb_soa_chunk + names
 
 struct ingest_stats {
 	u64 mapped_reads; std::vector<u64> mapped_viral_reads_by_contig; u64 malformed, missing_hi_tag, records, multimapper_pairs /* neighbours with the same read name */; bool no_chimeric_reads;
+	u64 chimeric_records, chimeric_malformed, chimeric_total; // the -c file: records, fragments the first malformed pass rejected / kept (0 without one)
 	double t_inflate, t_parse, t_finalize;
 };
 
@@ -79,6 +80,8 @@ struct ingest_options {
 	bool external_duplicate_marking; u32 max_itd_length; std::string interesting_contigs, viral_contigs; int threads /* inflate */;
 	struct ::arb_ctx* scan_ctx; // device context that runs the record loop and builds the fragment table
 	std::function<void()> after_header; // once the BAM header has grown the contig table: the contigs and the gene index must reach scan_ctx before the records
+	std::string chimeric_path; // -c file, read before the main file (empty: none)
+	std::function<void(u64)> chimeric_done; // with a -c file: its part is complete (no error of it is left); the argument is its progress line's total
 };
 
 // reads the BAM, fills `out` (name order, slots normalised, multimappers marked); throws std::runtime_error on fatal input errors

@@ -50,6 +50,8 @@ void pipeline::ingest() {
 	io.interesting_contigs = opt.interesting_contigs; io.viral_contigs = opt.viral_contigs; io.threads = threads;
 	attach_device(); io.scan_ctx = ctx;
 	io.after_header = [this]() { begin_upload(); send_annotation(); }; // the read-through test queries the GTF's genes (before the dummy genes of annotate())
+	io.chimeric_path = opt.chimeric_file;
+	io.chimeric_done = [this](u64 total) { std::ostringstream s; s << "Reading chimeric alignments from '" << opt.chimeric_file << "' (total=" << total << ")"; say(s.str()); };
 	read_chimeric_alignments(opt.bam_file, ref, io, frags, coverage, istats);
 	std::ostringstream s; s << "Reading chimeric alignments from '" << opt.bam_file << "' (total=" << frags.n << ")";
 	say(s.str());

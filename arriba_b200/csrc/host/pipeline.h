@@ -38,6 +38,7 @@ struct run_options { // options_t (options.hpp:25-69) restricted to what this im
 	std::string blacklist_file; // -b (empty: none)
 	std::string known_fusions_file, tags_file; // -k, -t (empty: none)
 	std::string protein_domains_file; // -p (empty: none)
+	std::string chimeric_file; // -c: STAR's Chimeric.out.sam (empty: none)
 	run_options();
 };
 

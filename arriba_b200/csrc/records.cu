@@ -1,5 +1,6 @@
 // records.cu -- the reference's record loop on the device (functors: records_hd.h).
 //   records_begin  : the BAM header's contig map, the contig flags, the coverage windows' layout,
+//   records_source : a separate chimeric file (-c) ahead of the main file: which file the following chunks belong to, and its header's contig map,
 //   records_chunk  : per chunk of inflated payload: copy it up behind the unfinished record of the previous chunk, find the records (bamscan.cu), classify
 //                    them and append the kept ones to the record store, which lives across chunks (mates and supplementaries of one key may sit anywhere
 //                    in the file),
@@ -8,6 +9,7 @@
 //                    counts into packed 16-bit windows, and bring the windows and the counters back.
 #include <cstdlib>
 #include <cstdio>
+#include <type_traits>
 #include "engine.h"
 #include "records_hd.h"
 #include "fragtable_hd.h"
@@ -54,12 +56,27 @@ void engine::records_begin(const u16* tid_to_contig, u32 n_tid, const u8* intere
 	rec_counters.ensure((size_t) REC_CTR_VIRAL + n_contigs); rec_counters.zero(ex, (size_t) REC_CTR_VIRAL + n_contigs);
 	const u64 none = ~(u64) 0; rec_error.upload(ex, &none, 1);
 	rec_n = 0; rec_arena_used = 0; rec_carry = 0; rec_carry_at = 0; rec_error_record.clear();
+	rec_src_chimeric = rec_has_chimeric = false; rec_pos_base = rec_pos_end = rec_chimeric_end = 0;
 	// test hook: keys share their hash far more often than 64-bit hashes ever do, so that runs of one hash hold many keys
 	const char* bits = getenv("ARB_KEY_HASH_BITS");
 	rec_hash_mask = bits && atoi(bits) > 0 && atoi(bits) < 64 ? ((u64) 1 << atoi(bits)) - 1 : ~(u64) 0;
 	timings.bam_scan_ms = 0; timings.h2d_ms = 0; timings.h2d_bytes = 0;
 	timings.rec_chunk_copy_ms = timings.rec_chunk_kernels_ms = timings.rec_sort_ms = timings.rec_count_ms = timings.rec_scan_ms = timings.rec_write_ms = timings.rec_download_ms = timings.rec_text_parse_ms = 0;
 	rec_open = true;
+}
+
+// The records of the chunks that follow belong to the -c file (chimeric_file) or to the main file, whose header maps its references by tid_to_contig.
+// Every file's positions start behind those of the files before it (first_position): the store then orders a key's records by file, then by position,
+// and the earliest record error is the one the reference meets first.
+void engine::records_source(bool chimeric_file, const u16* tid_to_contig, u32 n_tid, u64* first_position) {
+	if (!rec_open) throw arb_error("arb_records_source without arb_records_begin");
+	if (rec_carry) throw arb_error("arb_records_source: the previous file ended inside a record");
+	if (rec_has_chimeric && !rec_src_chimeric && chimeric_file) throw arb_error("arb_records_source: the -c file must come before the main file");
+	if (!chimeric_file && rec_src_chimeric) rec_chimeric_end = rec_pos_end;
+	rec_has_chimeric = rec_has_chimeric || chimeric_file; rec_src_chimeric = chimeric_file;
+	rec_pos_base = rec_pos_end; *first_position = rec_pos_base;
+	rec_n_tid = n_tid; rec_tid.upload(ex, tid_to_contig, n_tid); rec_tid.ensure(1);
+	rec_text_staged = 0; rec_carry_at = 0;
 }
 
 // the chunk goes to the device behind the unfinished record (or line) at the end of the previous one; returns the bytes of bam_buf now in use
@@ -86,7 +103,7 @@ void engine::records_chunk(const u8* chunk, u64 bytes, u64 first, u64 chunk_pos,
 	const u64 total = records_upload(chunk, bytes);
 	timings.rec_chunk_copy_ms += t_copy.stop();
 	stage_timer t_kernels(ex);
-	const u64 buf_pos = chunk_pos - (total - bytes);
+	const u64 buf_pos = rec_pos_base + chunk_pos - (total - bytes);
 	u64 consumed = 0; u32 R = 0;
 	dbuf<u32> rec_off;
 	bam_scan(bam_buf.ptr(), total, first_record, (i32) rec_n_tid, rec_off, &consumed, &R, malformed);
@@ -104,8 +121,14 @@ void engine::records_store(const dbuf<u8>& B, u64 buf_pos, u64 total, const u32*
 	// classify, then append the kept records to the store
 	dbuf<u32> bytes_of((size_t) R + 1), kept((size_t) R + 1); dbuf<u64> hash(R); dbuf<i64> hit(R); dbuf<u8> sa(R);
 	const rec_chunk_view cv = {B.ptr(), rec_off, buf_pos, rec_tid.ptr(), (i32) rec_n_tid, annot.contig_len.ptr(), rec_interesting.ptr()};
-	rec_extract_fn xf = {cv, rec_hash_mask, bytes_of.ptr(), kept.ptr(), hash.ptr(), hit.ptr(), sa.ptr(), rec_counters.ptr(), rec_error.ptr()};
-	for_each(ex, R, xf);
+	rec_pos_end = std::max(rec_pos_end, buf_pos + total);
+	if (rec_src_chimeric) {
+		rec_extract_t<true> xf = {cv, rec_hash_mask, bytes_of.ptr(), kept.ptr(), hash.ptr(), hit.ptr(), sa.ptr(), rec_counters.ptr(), rec_error.ptr()};
+		for_each(ex, R, xf);
+	} else {
+		rec_extract_fn xf = {cv, rec_hash_mask, bytes_of.ptr(), kept.ptr(), hash.ptr(), hit.ptr(), sa.ptr(), rec_counters.ptr(), rec_error.ptr()};
+		for_each(ex, R, xf);
+	}
 	exclusive_scan_u32(ex, bytes_of.ptr(), bytes_of.ptr(), R); exclusive_scan_u32(ex, kept.ptr(), kept.ptr(), R);
 	u32 add_bytes = 0, add_items = 0;
 	bytes_of.download(ex, &add_bytes, 1, R); kept.download(ex, &add_items, 1, R);
@@ -171,68 +194,83 @@ void engine::records_finish(u16* const* coverage, u8* const* starts, u8* const* 
 	dbuf<u32> seg_begin((size_t) S + 1);
 	rec_seg_begin_fn bf = {seg_at.ptr(), n, seg_begin.ptr()}; for_each(ex, n + 1, bf);
 	timings.rec_sort_ms = t_sort.stop();
-	stage_timer t_count(ex);
-	// 3. replay: count (sets of up to 32 gene ids, the few segments that need more: 1024), scan, write
-	dbuf<u8> big((size_t) S + 1); big.zero(ex, (size_t) S + 1);
-	const u32 stride = (S + 4) & ~3u; // S + 1 entries per row, rows 16-byte aligned (the scan loads four items at a time)
-	dbuf<u32> tally((size_t) RS_N * stride), big_list((size_t) S + 1), n_big(1);
-	dbuf<u64> search_log((size_t) n + 1); // what the counting pass's searches decided, per store position (written before it is read: no zeroing)
-	const rec_store_view sv = {rec_arena.ptr(), rec_at.ptr(), rec_pos.ptr(), rec_hit.ptr(), rec_sa.ptr(), order.ptr()};
-	rec_cov_view cov = {NULL, rec_cov_starts.ptr(), rec_cov_ends.ptr(), rec_cov_off.ptr(), rec_cov_n.ptr(), rec_n_contigs}; // counts: writing pass only
-	const rec_params prm = {rec_max_itd, (u8) (rec_external_dup ? 1 : 0), rec_viral.ptr()};
-	const annot_view an = annot.view();
-	rec_replay_fn<32> small = {sv, seg_begin.ptr(), NULL, big.ptr(), an, prm, cov, tally.ptr(), tally.ptr(), stride, NULL, NULL, NULL, NULL, NULL, search_log.ptr(), rec_counters.ptr(), rec_error.ptr(), false};
-	for_each(ex, S, small);
-	n_big.zero(ex, 1);
-	rec_big_list_fn lf = {big.ptr(), big_list.ptr(), n_big.ptr()}; for_each(ex, S, lf);
-	u32 B = 0; n_big.download(ex, &B, 1);
-	rec_replay_fn<1024> large = {sv, seg_begin.ptr(), big_list.ptr(), big.ptr(), an, prm, cov, tally.ptr(), tally.ptr(), stride, NULL, NULL, NULL, NULL, NULL, search_log.ptr(), rec_counters.ptr(), rec_error.ptr(), false};
-	for_each(ex, B, large);
-	rec_error.download(ex, error, 1);
-	timings.rec_count_ms = t_count.stop();
-	if (*error != ~(u64) 0) { timings.bam_scan_ms += t_all.stop(); return; }
-	stage_timer t_scan(ex);
-	// The scans are 32-bit. A prefix sum that passes 2^32 wraps, and every wrap shows as a step down between neighbours (each tally is < 2^32): counted,
-	// the true totals follow, and a sample whose pools the table cannot address stops here, before anything is written.
-	for (u32 q = 0; q < RS_N; ++q) exclusive_scan_u32(ex, tally.ptr() + (size_t) q * stride, tally.ptr() + (size_t) q * stride, S);
-	dbuf<u32> wraps(RS_N); wraps.zero(ex, RS_N);
-	rec_wrap_fn wf = {tally.ptr(), stride, S, wraps.ptr()}; for_each(ex, RS_N * S, wf);
-	u32 tot[RS_N], n_wraps[RS_N];
-	for (u32 q = 0; q < RS_N; ++q) tally.download(ex, tot + q, 1, (size_t) q * stride + S);
-	wraps.download(ex, n_wraps, RS_N);
-	timings.rec_scan_ms = t_scan.stop();
-	{
-		u64 total[RS_N], limit[RS_N] = {(u64) 1 << 30 /* fragment ids */, (u64) 1 << 31 /* i32 alignment links */, (u64) 1 << 32, (u64) 1 << 32, (u64) 1 << 32};
-		const char* hook = getenv("ARB_REPLAY_POOL_LIMIT"); // test hook: the limits lowered, so that a small sample reaches them
-		bool over = false;
-		for (u32 q = 0; q < RS_N; ++q) {
-			total[q] = (u64) n_wraps[q] << 32 | tot[q];
-			if (hook && atoll(hook) > 0) limit[q] = std::min<u64>(limit[q], (u64) atoll(hook));
-			over = over || total[q] >= limit[q];
+	// 3. replay, with the -c file's steps compiled in only when there is one
+	dbuf<u64> cov_counts(rec_cov_windows + 2);
+	dbuf<u32> chimeric_counts(2); chimeric_counts.zero(ex, 2); // the -c fragments the first malformed pass rejects / keeps (counting pass)
+	auto replay = [&](auto chimeric_file) -> bool { // false: the counting pass found a fatal error
+		constexpr bool C = decltype(chimeric_file)::value;
+		stage_timer t_count(ex);
+		// count (sets of up to 32 gene ids, the few segments that need more: 1024), scan, write
+		dbuf<u8> big((size_t) S + 1); big.zero(ex, (size_t) S + 1);
+		const u32 stride = (S + 4) & ~3u; // S + 1 entries per row, rows 16-byte aligned (the scan loads four items at a time)
+		dbuf<u32> tally((size_t) RS_N * stride), big_list((size_t) S + 1), n_big(1);
+		dbuf<u64> search_log((size_t) n + 1); // what the counting pass's searches decided, per store position (written before it is read: no zeroing)
+		if (rec_src_chimeric) rec_chimeric_end = rec_pos_end; // the -c file was the last one (no main file followed)
+		const rec_store_view sv = {rec_arena.ptr(), rec_at.ptr(), rec_pos.ptr(), rec_hit.ptr(), rec_sa.ptr(), order.ptr(), rec_chimeric_end};
+		rec_cov_view cov = {NULL, rec_cov_starts.ptr(), rec_cov_ends.ptr(), rec_cov_off.ptr(), rec_cov_n.ptr(), rec_n_contigs}; // counts: writing pass only
+		const rec_params prm = {rec_max_itd, (u8) (rec_external_dup ? 1 : 0), rec_viral.ptr()};
+		const annot_view an = annot.view();
+		rec_replay_fn<32, C> small = {sv, seg_begin.ptr(), NULL, big.ptr(), an, prm, cov, tally.ptr(), tally.ptr(), stride, NULL, NULL, NULL, NULL, NULL, search_log.ptr(), rec_counters.ptr(), rec_error.ptr(), false, chimeric_counts.ptr()};
+		for_each(ex, S, small);
+		n_big.zero(ex, 1);
+		rec_big_list_fn lf = {big.ptr(), big_list.ptr(), n_big.ptr()}; for_each(ex, S, lf);
+		u32 B = 0; n_big.download(ex, &B, 1);
+		rec_replay_fn<1024, C> large = {sv, seg_begin.ptr(), big_list.ptr(), big.ptr(), an, prm, cov, tally.ptr(), tally.ptr(), stride, NULL, NULL, NULL, NULL, NULL, search_log.ptr(), rec_counters.ptr(), rec_error.ptr(), false, chimeric_counts.ptr()};
+		for_each(ex, B, large);
+		rec_error.download(ex, error, 1);
+		timings.rec_count_ms = t_count.stop();
+		if (C) { u32 c[2]; chimeric_counts.download(ex, c, 2); ft_chimeric[0] = c[0]; ft_chimeric[1] = c[1]; }
+		else ft_chimeric[0] = ft_chimeric[1] = 0;
+		if (*error != ~(u64) 0) return false;
+		stage_timer t_scan(ex);
+		// The scans are 32-bit. A prefix sum that passes 2^32 wraps, and every wrap shows as a step down between neighbours (each tally is < 2^32): counted,
+		// the true totals follow, and a sample whose pools the table cannot address stops here, before anything is written.
+		for (u32 q = 0; q < RS_N; ++q) exclusive_scan_u32(ex, tally.ptr() + (size_t) q * stride, tally.ptr() + (size_t) q * stride, S);
+		dbuf<u32> wraps(RS_N); wraps.zero(ex, RS_N);
+		rec_wrap_fn wf = {tally.ptr(), stride, S, wraps.ptr()}; for_each(ex, RS_N * S, wf);
+		u32 tot[RS_N], n_wraps[RS_N];
+		for (u32 q = 0; q < RS_N; ++q) tally.download(ex, tot + q, 1, (size_t) q * stride + S);
+		wraps.download(ex, n_wraps, RS_N);
+		timings.rec_scan_ms = t_scan.stop();
+		{
+			u64 total[RS_N], limit[RS_N] = {(u64) 1 << 30 /* fragment ids */, (u64) 1 << 31 /* i32 alignment links */, (u64) 1 << 32, (u64) 1 << 32, (u64) 1 << 32};
+			const char* hook = getenv("ARB_REPLAY_POOL_LIMIT"); // test hook: the limits lowered, so that a small sample reaches them
+			bool over = false;
+			for (u32 q = 0; q < RS_N; ++q) {
+				total[q] = (u64) n_wraps[q] << 32 | tot[q];
+				if (hook && atoll(hook) > 0) limit[q] = std::min<u64>(limit[q], (u64) atoll(hook));
+				over = over || total[q] >= limit[q];
+			}
+			if (over) {
+				char m[400];
+				snprintf(m, sizeof(m), "the sample is too large for one fragment table: %llu fragments (limit %llu), %llu alignments (limit %llu), %llu name bytes (limit %llu), "
+				         "%llu CIGAR operations (limit %llu), %llu sequence bytes (limit %llu)",
+				         (unsigned long long) total[RS_FRAGS], (unsigned long long) limit[RS_FRAGS], (unsigned long long) total[RS_ALNS], (unsigned long long) limit[RS_ALNS],
+				         (unsigned long long) total[RS_NAMES], (unsigned long long) limit[RS_NAMES], (unsigned long long) total[RS_CIGARS], (unsigned long long) limit[RS_CIGARS],
+				         (unsigned long long) total[RS_UNITS] * 16, (unsigned long long) limit[RS_UNITS] * 16);
+				throw arb_error(m);
+			}
 		}
-		if (over) {
-			char m[400];
-			snprintf(m, sizeof(m), "the sample is too large for one fragment table: %llu fragments (limit %llu), %llu alignments (limit %llu), %llu name bytes (limit %llu), "
-			         "%llu CIGAR operations (limit %llu), %llu sequence bytes (limit %llu)",
-			         (unsigned long long) total[RS_FRAGS], (unsigned long long) limit[RS_FRAGS], (unsigned long long) total[RS_ALNS], (unsigned long long) limit[RS_ALNS],
-			         (unsigned long long) total[RS_NAMES], (unsigned long long) limit[RS_NAMES], (unsigned long long) total[RS_CIGARS], (unsigned long long) limit[RS_CIGARS],
-			         (unsigned long long) total[RS_UNITS] * 16, (unsigned long long) limit[RS_UNITS] * 16);
-			throw arb_error(m);
-		}
+		stage_timer t_write(ex);
+		pool_frags.ensure(tot[RS_FRAGS]); pool_alns.ensure(tot[RS_ALNS]); pool_names.ensure(tot[RS_NAMES]); pool_cigars.ensure(tot[RS_CIGARS]); pool_seqs.ensure((size_t) tot[RS_UNITS] * 16);
+		cov_counts.zero(ex, rec_cov_windows + 2);
+		small.write = large.write = true;
+		small.cov.counts = large.cov.counts = cov_counts.ptr();
+		small.frags = large.frags = pool_frags.ptr(); small.alns = large.alns = pool_alns.ptr(); small.names = large.names = pool_names.ptr();
+		small.cigars = large.cigars = pool_cigars.ptr(); small.seqs = large.seqs = pool_seqs.ptr();
+		for_each(ex, S, small);
+		for_each(ex, B, large);
+		const u64 base[2 * FT_POOLS] = {0, tot[RS_FRAGS], 0, tot[RS_ALNS], 0, tot[RS_NAMES], 0, tot[RS_CIGARS], 0, (u64) tot[RS_UNITS] * 16};
+		pool_base.upload(ex, base, 2 * FT_POOLS);
+		pool_workers = 1;
+		timings.rec_write_ms = t_write.stop();
+		return true;
+	};
+	if (!(rec_has_chimeric ? replay(std::true_type()) : replay(std::false_type()))) {
+		// the counters so far: with a -c file, REC_CTR_CHIMERIC tells whether it had chimeric reads (its error comes before the main file's)
+		rec_counters.download(ex, counters, (size_t) REC_CTR_VIRAL + rec_n_contigs);
+		timings.bam_scan_ms += t_all.stop(); return;
 	}
-	stage_timer t_write(ex);
-	pool_frags.ensure(tot[RS_FRAGS]); pool_alns.ensure(tot[RS_ALNS]); pool_names.ensure(tot[RS_NAMES]); pool_cigars.ensure(tot[RS_CIGARS]); pool_seqs.ensure((size_t) tot[RS_UNITS] * 16);
-	dbuf<u64> cov_counts(rec_cov_windows + 2); cov_counts.zero(ex, rec_cov_windows + 2);
-	small.write = large.write = true;
-	small.cov.counts = large.cov.counts = cov_counts.ptr();
-	small.frags = large.frags = pool_frags.ptr(); small.alns = large.alns = pool_alns.ptr(); small.names = large.names = pool_names.ptr();
-	small.cigars = large.cigars = pool_cigars.ptr(); small.seqs = large.seqs = pool_seqs.ptr();
-	for_each(ex, S, small);
-	for_each(ex, B, large);
-	const u64 base[2 * FT_POOLS] = {0, tot[RS_FRAGS], 0, tot[RS_ALNS], 0, tot[RS_NAMES], 0, tot[RS_CIGARS], 0, (u64) tot[RS_UNITS] * 16};
-	pool_base.upload(ex, base, 2 * FT_POOLS);
-	pool_workers = 1;
-	timings.rec_write_ms = t_write.stop();
 	stage_timer t_download(ex);
 	// 4. the by-products: the counts saturated into packed 16-bit windows, then every contig's windows straight into the caller's arrays (the
 	// 16-bit counters lie in their 32-bit words in little-endian order, i.e. as a plain u16 array)

@@ -1,7 +1,9 @@
-// records_hd.h -- what the reference's record loop does with every BAM record (read_chimeric_alignments.cpp:611-749 for -x input), as host/device code
-// (records.cu drives it; the CPU stand-in runs the same functors).
+// records_hd.h -- what the reference's record loop does with every BAM record (read_chimeric_alignments.cpp:611-749), as host/device code
+// (records.cu drives it; the CPU stand-in runs the same functors). The main file (-x) and, ahead of it, a separate chimeric file (-c, STAR's
+// Chimeric.out.sam) go into one record store; the replay runs both files' loops for every key.
 //   rec_extract_fn : one thread per record of a chunk: the records the loop skips, HI and SA, the two validity checks, the key hash and the size of the
-//                    compact copy that the record store keeps across chunks (fixed fields with the contig id, name, CIGAR, nt16 sequence),
+//                    compact copy that the record store keeps across chunks (fixed fields with the contig id, name, CIGAR, nt16 sequence);
+//                    rec_extract_t<true> is the -c file's variant,
 //   rec_store_fn   : the copy itself,
 //   rec_replay_fn  : one thread per run of equal key hashes (the store sorted stably by hash: file order inside a run): every key of the run replays the
 //                    loop's steps in file order -- supplementaries, discordant mates, proper pairs (each record alternates between waiting and pairing),
@@ -14,14 +16,16 @@
 #include "model.h"
 #include "prims.h"
 #include "annot_hd.h"
+#include "fragtable_hd.h"
 #include "../../include/arriba_b200.h"
 
 namespace arb {
 
 enum { BF_PAIRED = 1, BF_PROPER = 2, BF_UNMAP = 4, BF_MUNMAP = 8, BF_REVERSE = 16, BF_READ1 = 64, BF_SECONDARY = 256, BF_DUP = 1024, BF_SUPPLEMENTARY = 2048 };
 // fatal record errors, by file position (the smallest position wins: the reference reads serially); the host raises them with their texts (ingest.cpp)
-enum { REC_ERR_LOAD = 1, REC_ERR_CIGAR = 2, REC_ERR_BEYOND = 3, REC_ERR_ANNOTATION = 4 };
-// device counters of the loop's by-products: [REC_CTR_VIRAL + contig] = pristine reads per viral contig
+enum { REC_ERR_LOAD = 1, REC_ERR_CIGAR = 2, REC_ERR_BEYOND = 3, REC_ERR_ANNOTATION = 4, REC_ERR_UNMAPPED = 5 /* a -c record without a reference */ };
+// device counters of the loop's by-products: [REC_CTR_VIRAL + contig] = pristine reads per viral contig. REC_CTR_CHIMERIC: the loop added an alignment
+// (with a -c file only the -c file's loop adds them outside read-through and tandem-duplication fragments; the -x file's loop then never sets it)
 enum { REC_CTR_MAPPED = 0, REC_CTR_MALFORMED = 1, REC_CTR_MISSING_HI = 2, REC_CTR_CHIMERIC = 3, REC_CTR_VIRAL = 4 };
 
 ARB_HD u32 rec_rd32(const u8* p) { return (u32) p[0] | (u32) p[1] << 8 | (u32) p[2] << 16 | (u32) p[3] << 24; }
@@ -171,7 +175,10 @@ struct rec_chunk_view {
 	const u8* B; const u32* rec_off; u64 buf_pos /* file position (inflated stream) of B[0] */;
 	const u16* tid_to_contig; i32 n_tid; const u32* contig_len; const u8* interesting;
 };
-struct rec_extract_fn {
+// CHIMERIC_FILE: the records of a -c file (read_chimeric_alignments.cpp:611-623 with separate_chimeric_bam_file set, is_rna_bam_file not): none is skipped
+// (a record without a reference is an error that names it: the reference indexes tid_to_contig[-1]), HI is not read (every key is "<qname>,1"), nothing is
+// counted (the call's interesting_tids stays all false), and the SA tag plays no part.
+template <bool CHIMERIC_FILE> struct rec_extract_t {
 	rec_chunk_view c; u64 hash_mask;
 	u32* bytes /* compact size, 0 = not kept */; u32* kept; u64* hash; i64* hit; u8* has_sa; u64* counters; u64* error;
 	ARB_HD void fail(u32 i, u32 kind) const { rec_atomic_min_u64(error, (c.buf_pos + c.rec_off[i]) << 3 | kind); }
@@ -180,22 +187,27 @@ struct rec_extract_fn {
 		const u8* p = c.B + c.rec_off[i];
 		rec_t r;
 		if (!rec_parse(p + 4, rec_rd32(p), r)) { fail(i, REC_ERR_LOAD); return; }
-		if (rec_skipped(r)) return;
 		i64 hit_index = 1;
-		const u8* hi = rec_find_aux(r, 'H', 'I');
-		if (hi) hit_index = rec_aux_int(hi);
-		else if (r.flag & BF_SECONDARY) { rec_count_one(&counters[REC_CTR_MISSING_HI]); return; }
+		if (CHIMERIC_FILE) {
+			if (r.tid < 0) { fail(i, REC_ERR_UNMAPPED); return; }
+		} else {
+			if (rec_skipped(r)) return;
+			const u8* hi = rec_find_aux(r, 'H', 'I');
+			if (hi) hit_index = rec_aux_int(hi);
+			else if (r.flag & BF_SECONDARY) { rec_count_one(&counters[REC_CTR_MISSING_HI]); return; }
+		}
 		if (r.tid < 0 || r.tid >= c.n_tid) { fail(i, REC_ERR_LOAD); return; }
 		const u32 contig = c.tid_to_contig[r.tid];
 		i64 query_span;
 		const u32 bad = rec_validate(r, c.contig_len[contig], query_span);
 		if (bad) { fail(i, bad); return; }
-		if (!(r.flag & BF_SUPPLEMENTARY) && c.interesting[contig]) rec_count_one(&counters[REC_CTR_MAPPED]);
+		if (!CHIMERIC_FILE && !(r.flag & BF_SUPPLEMENTARY) && c.interesting[contig]) rec_count_one(&counters[REC_CTR_MAPPED]);
 		bytes[i] = r.compact_bytes(); kept[i] = 1;
 		hash[i] = rec_key_hash(r.qname(), r.name_len(), hit_index) & hash_mask; hit[i] = hit_index;
-		has_sa[i] = rec_find_aux(r, 'S', 'A') != 0;
+		has_sa[i] = !CHIMERIC_FILE && rec_find_aux(r, 'S', 'A') != 0;
 	}
 };
+typedef rec_extract_t<false> rec_extract_fn;
 struct rec_store_fn { // record i of the chunk -> store item n_stored + kept[i] at byte arena_used + at[i] (at, kept: exclusive scans of the sizes / the kept flags)
 	rec_chunk_view c; const u32* at; const u32* kept; const u64* hash; const i64* hit; const u8* has_sa;
 	u64 n_stored, arena_used; u8* arena; u64* s_at; u64* s_pos; u32* s_hash_lo; u32* s_hash_hi; i64* s_hit; u8* s_sa;
@@ -216,6 +228,8 @@ struct rec_store_fn { // record i of the chunk -> store item n_stored + kept[i] 
 // ------------------------------------------------------------------------------------------- after the last chunk: replay
 struct rec_store_view {
 	const u8* arena; const u64* at; const u64* pos; const i64* hit; const u8* sa; const u32* order /* sorted by key hash, file order inside a hash */;
+	u64 chimeric_end; // records at positions below it come from a -c file (which precedes the main file: a key's -c records come first)
+	ARB_HD bool from_chimeric_file(u32 k) const { return pos[k] < chimeric_end; }
 	ARB_HD void get(u32 k, rec_t& r) const { const u8* p = arena + at[k]; rec_parse(p, 0xFFFFFFFFu, r, false); r.aux = r.aux_end = 0; }
 	ARB_HD bool same_key(u32 a, u32 b) const {
 		if (hit[a] != hit[b]) return false;
@@ -351,6 +365,7 @@ struct rec_emit {
 	arb_pool_fragment* frags; arb_pool_alignment* alns; char* names; u32* cigars; u8* seqs;
 	u32 base[RS_N]; u32 n[RS_N];
 	i32 id[2]; // fragment of the key / of the key's ITD, -1 before it is created
+	u8 chimeric_file; // the fragments created now come from a -c file
 	ARB_HD bool writing() const { return frags != 0; }
 	// fragment(name, &created)
 	ARB_HD u32 fragment(const rec_t& named, i64 hit_index, int itd, bool* created) {
@@ -365,7 +380,7 @@ struct rec_emit {
 			for (u32 x = 0; x < nd; ++x) d[nn + 1 + x] = digits[x];
 			if (itd) { d[nn + 1 + nd] = 'I'; d[nn + 2 + nd] = 'T'; d[nn + 3 + nd] = 'D'; }
 			arb_pool_fragment& g = frags[f];
-			g.name_off = base[RS_NAMES] + n[RS_NAMES]; g.name_len = len; g.head = g.tail = -1; g.count = 0; g.single_end = 0; g.duplicate = 0;
+			g.name_off = base[RS_NAMES] + n[RS_NAMES]; g.name_len = len; g.head = g.tail = -1; g.count = 0; g.single_end = 0; g.duplicate = 0; g.chimeric_file = chimeric_file;
 		}
 		n[RS_NAMES] += len;
 		id[itd] = (i32) f;
@@ -479,16 +494,27 @@ ARB_HD rec_genes rec_genes_at(const region_index_view& ix, u32 contig, i32 pos) 
 	return g;
 }
 
+// What the replay keeps per key while it walks the key's records
+struct rec_key_state {
+	i32 waiting, waiting_c; // the first mate of a proper pair waiting for the second, in the main file's / the -c file's loop (-1: none)
+	u32 c_n, c_rec[3];      // the alignments of the key's -c fragment (store items of the first three)
+	u8 c_single_end; bool c_judged, c_kept; // c_kept: the first malformed pass keeps the -c fragment (once c_judged)
+};
+// the CIGAR operations of a stored record, read where they lie (the store keeps them behind the name, 4-byte alignment not guaranteed)
+struct rec_cigar_ops { const u8* raw; ARB_HD u32 operator[](u32 k) const { return rec_rd32(raw + 4 * k); } };
+
 // One thread per segment (run of equal key hashes). CAP bounds the gene sets of the read-through test, as the reference's fixed-capacity sets do: a segment
 // whose sets exceed 32 ids is left untouched and marked in `big` for a second launch with the reference's capacity (1024), where more is the reference's
 // fatal error. The sets are read in place from the gene index; CAP only decides which launch a segment belongs to.
 // Counting pass (write == false): the searches, their log, the segment's tallies. Writing pass: the pools, the coverage, the counters.
-template <int CAP> struct rec_replay_fn {
+// CHIMERIC_FILE: a -c file precedes the main file (its steps are compiled into these launches only: the launches of a run without one keep their registers).
+template <int CAP, bool CHIMERIC_FILE = false> struct rec_replay_fn {
 	rec_store_view s; const u32* seg_begin; const u32* list /* segments of this launch, NULL: all */; u8* big;
 	annot_view an; rec_params prm; rec_cov_view cov;
 	u32* tally /* RS_N rows of `stride` entries, one per segment */; const u32* bases /* the rows after their exclusive scans */; u32 stride;
 	arb_pool_fragment* frags; arb_pool_alignment* alns; char* names; u32* cigars; u8* seqs;
 	u64* log /* per store position: what the searches decided */; u64* counters; u64* error; bool write;
+	u32* chimeric /* counting pass with a -c file: the keys' -c fragments that the first malformed pass rejects / keeps */;
 
 	// the decision of the read-through test (read_chimeric_alignments.cpp:93-193) as a log entry; returns false and marks the segment when a gene set exceeds CAP
 	ARB_HD bool decide_read_through(u32 k, const rec_t* a, const rec_t* b, u64& decision) const {
@@ -540,28 +566,74 @@ template <int CAP> struct rec_replay_fn {
 		return true;
 	}
 
-	// one record of a key, in file order (read_chimeric_alignments.cpp:611-749); waiting: the key's first mate of a proper pair (-1: none)
-	ARB_HD bool process(rec_emit& e, u32 k, i32& waiting) const {
+	// A -c record (read_chimeric_alignments.cpp:627-631, 657-681, separate_chimeric_bam_file without is_rna_bam_file): a secondary alignment (0x100) is
+	// added as a supplementary one at once; mates are collated in the -c file's own slot and added as (this record, its waiting mate); single-end records
+	// are added as they come. A mate still waiting after the key's last -c record is dropped. No search, no coverage.
+	ARB_HD void chimeric_add(rec_emit& e, rec_key_state& st, u32 k, const rec_t& r, bool supplementary) const {
+		e.add_alignment(e.fragment(r, s.hit[k], 0, 0), r, supplementary);
+		if (st.c_n < 3) st.c_rec[st.c_n] = k;
+		++st.c_n; st.c_single_end = !(r.flag & BF_PAIRED);
+	}
+	ARB_HD void process_chimeric(rec_emit& e, u32 k, const rec_t& r, rec_key_state& st) const {
+		e.chimeric_file = 1;
+		if (r.flag & BF_SECONDARY) chimeric_add(e, st, k, r, true);
+		else if (r.flag & BF_PAIRED) {
+			if (st.waiting_c < 0) { st.waiting_c = (i32) k; e.chimeric_file = 0; return; }
+			const u32 mk = (u32) st.waiting_c; st.waiting_c = -1;
+			rec_t mate; s.get(mk, mate);
+			chimeric_add(e, st, k, r, false); chimeric_add(e, st, mk, mate, false);
+		} else chimeric_add(e, st, k, r, false);
+		e.chimeric_file = 0;
+		counters[REC_CTR_CHIMERIC] = 1; // in both passes: when the main file has a fatal error, the counting pass alone tells whether the -c file had chimeric reads
+	}
+	// Does the first pass of remove_malformed_alignments (after the -c file) keep the key's -c fragment? The rule of the fragment table (ft_decide), on
+	// slots made from the stored records: a -c alignment is an unclipped copy of its record.
+	ARB_HD bool chimeric_fragment_kept(const rec_key_state& st) const {
+		const bool single_end = st.c_single_end != 0;
+		if (!ft_count_ok(single_end, st.c_n)) return false;
+		ft_slot_t<rec_cigar_ops> m[3];
+#pragma unroll
+		for (u32 x = 0; x < 3; ++x) {
+			if (x >= st.c_n) break;
+			rec_t r; s.get(st.c_rec[x], r);
+			const bool supplementary = r.flag & BF_SECONDARY;
+			m[x].contig = (u16) r.tid; m[x].supplementary = supplementary; m[x].first_in_pair = (r.flag & BF_READ1) ? 1 : 0; m[x].forward = !r.reverse();
+			m[x].start = r.pos; m[x].end = r.endpos() - 1; m[x].seq_len = supplementary ? 0 : (u32) r.l_seq; m[x].seq_off = 0;
+			m[x].cnt = r.n_cigar; m[x].ops.raw = r.cigar_raw; m[x].n_set = 0;
+		}
+		return ft_decide(single_end, st.c_n, m) != 0;
+	}
+
+	// one record of a key, in file order (read_chimeric_alignments.cpp:611-749): the -c file's records first, then the main file's. With a -c file the main
+	// file's loop adds no supplementary, discordant or SA-tagged alignment (it still counts coverage for them), and its read-through fragments are inserted
+	// only where the map holds no fragment of the key: the -c fragment counts only if the first malformed pass kept it.
+	ARB_HD bool process(rec_emit& e, u32 k, rec_key_state& st) const {
 		rec_t r; s.get(k, r);
+		if (CHIMERIC_FILE && s.from_chimeric_file(k)) { process_chimeric(e, k, r, st); return true; }
+		if (CHIMERIC_FILE && !st.c_judged) {
+			st.c_judged = true; st.c_kept = st.c_n > 0 && chimeric_fragment_kept(st);
+			if (st.c_n > 0 && !st.c_kept) e.id[0] = -1; // erased: a read-through fragment may take its name (the build drops the rejected one)
+		}
 		const i64 hit_index = s.hit[k];
 		if (r.flag & BF_SUPPLEMENTARY) {
+			if (CHIMERIC_FILE) return true;
 			if (clipped_at_correct_end(r)) e.add_alignment(e.fragment(r, hit_index, 0, 0), r, true);
 			else if (write) rec_atomic_add_u64(&counters[REC_CTR_MALFORMED], 1);
 			if (write) counters[REC_CTR_CHIMERIC] = 1;
 			return true;
 		}
 		if ((r.flag & BF_PAIRED) && !(r.flag & BF_PROPER)) { // discordant mate
-			e.add_alignment(e.fragment(r, hit_index, 0, 0), r, false);
+			if (!CHIMERIC_FILE) e.add_alignment(e.fragment(r, hit_index, 0, 0), r, false);
 			if (write) {
-				counters[REC_CTR_CHIMERIC] = 1;
+				if (!CHIMERIC_FILE) counters[REC_CTR_CHIMERIC] = 1;
 				if (!prm.external_duplicate_marking || !(r.flag & BF_DUP)) add_coverage(cov, r, 0, true, true); // all flag bits cleared (`flag &= !BAM_FPAIRED`)
 			}
 			return true;
 		}
 		rec_t mate; const rec_t* m = 0; u32 mk = 0;
 		if (r.flag & BF_PAIRED) { // the first mate of a proper pair waits for the second
-			if (waiting < 0) { waiting = (i32) k; return true; }
-			mk = (u32) waiting; waiting = -1;
+			if (st.waiting < 0) { st.waiting = (i32) k; return true; }
+			mk = (u32) st.waiting; st.waiting = -1;
 			s.get(mk, mate); m = &mate;
 		}
 		u64 decision = write ? log[k] : 0;
@@ -586,10 +658,12 @@ template <int CAP> struct rec_replay_fn {
 		}
 		bool is_read_through = false;
 		if ((s.sa[k] && clipped_at_correct_end(r)) || (m && s.sa[mk] && clipped_at_correct_end(*m))) {
-			const u32 f = e.fragment(r, hit_index, 0, 0);
-			e.add_alignment(f, r, false);
-			if (m) e.add_alignment(f, *m, false);
-			if (write) counters[REC_CTR_CHIMERIC] = 1;
+			if (!CHIMERIC_FILE) {
+				const u32 f = e.fragment(r, hit_index, 0, 0);
+				e.add_alignment(f, r, false);
+				if (m) e.add_alignment(f, *m, false);
+				if (write) counters[REC_CTR_CHIMERIC] = 1;
+			}
 		} else if (!is_tandem) {
 			if (!write) {
 				u64 rt;
@@ -611,9 +685,10 @@ template <int CAP> struct rec_replay_fn {
 		const u32 seg = list ? list[i] : i;
 		if (!list && big[seg]) return; // left to the launch with the larger sets
 		rec_emit e;
-		e.frags = write ? frags : 0; e.alns = alns; e.names = names; e.cigars = cigars; e.seqs = seqs;
+		e.frags = write ? frags : 0; e.alns = alns; e.names = names; e.cigars = cigars; e.seqs = seqs; e.chimeric_file = 0;
 		for (u32 q = 0; q < RS_N; ++q) { e.base[q] = write ? bases[q * stride + seg] : 0; e.n[q] = 0; }
 		const u32 lo = seg_begin[seg], hi = seg_begin[seg + 1];
+		u32 c_rejected = 0, c_kept = 0;
 		// Every key of the segment (keys with one hash: names compared exactly), in the order of their first records. Quadratic in the segment's length:
 		// with 64-bit hashes a segment is one key's 2-4 records (keys sharing a hash are rare); only the ARB_KEY_HASH_BITS test hook makes segments long.
 		for (u32 x = lo; x < hi; ++x) {
@@ -622,14 +697,19 @@ template <int CAP> struct rec_replay_fn {
 			for (u32 y = lo; y < x && !seen; ++y) seen = s.same_key(s.order[y], kx);
 			if (seen) continue;
 			e.id[0] = e.id[1] = -1;
-			i32 waiting = -1; // still waiting at the end: dropped
+			rec_key_state st = {-1, -1, 0, {0, 0, 0}, 0, false, false}; // mates still waiting at the end: dropped
 			for (u32 y = x; y < hi; ++y) {
 				const u32 ky = s.order[y];
 				if (y != x && !s.same_key(kx, ky)) continue;
-				if (!process(e, ky, waiting)) { big[seg] = 1; return; }
+				if (!process(e, ky, st)) { big[seg] = 1; return; }
+			}
+			if (CHIMERIC_FILE && !write && st.c_n > 0) { // the first pass's verdict on the key's -c fragment, also for keys without main-file records
+				const bool kept = st.c_judged ? st.c_kept : chimeric_fragment_kept(st);
+				if (kept) ++c_kept; else ++c_rejected;
 			}
 		}
 		if (!write) for (u32 q = 0; q < RS_N; ++q) tally[q * stride + seg] = e.n[q];
+		if (CHIMERIC_FILE && !write) { if (c_rejected) atomic_add_u32(&chimeric[0], c_rejected); if (c_kept) atomic_add_u32(&chimeric[1], c_kept); } // the segment is complete
 	}
 };
 

@@ -65,7 +65,7 @@ void engine::records_text_chunk(const u8* chunk, u64 bytes, u64 first, u64 chunk
 	sam_write_fn sw = {lines, nm, at.ptr(), sam_stage.ptr()}; for_each(ex, L, sw);
 	timings.rec_text_parse_ms += t_parse.stop();
 	// 3. the record loop's classification and store, as for a BAM chunk
-	const u64 stage_pos = rec_text_staged;
+	const u64 stage_pos = rec_pos_base + rec_text_staged;
 	rec_text_staged += staged;
 	records_store(sam_stage, stage_pos, staged, at.ptr(), L, chunk_pos + bytes, error);
 	timings.rec_chunk_kernels_ms += t_kernels.stop();

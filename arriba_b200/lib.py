@@ -498,7 +498,7 @@ class RunOptions(C.Structure):
                 ("print_extra_info_for_discarded_fusions", C.c_int32), ("echo_progress", C.c_int32),
                 ("top_viral_contigs", C.c_uint32), ("viral_contig_min_covered_fraction", C.c_float),
                 ("genomic_breakpoints_file", C.c_char_p), ("max_genomic_breakpoint_distance", C.c_uint32), ("blacklist_file", C.c_char_p),
-                ("known_fusions_file", C.c_char_p), ("tags_file", C.c_char_p), ("protein_domains_file", C.c_char_p)]
+                ("known_fusions_file", C.c_char_p), ("tags_file", C.c_char_p), ("protein_domains_file", C.c_char_p), ("chimeric_file", C.c_char_p)]
 
 
 class RunStats(C.Structure):
@@ -506,7 +506,8 @@ class RunStats(C.Structure):
                 ("strandedness", C.c_int32), ("max_mate_gap", C.c_int32), ("fragment_length_ok", C.c_int32),
                 ("mate_gap_mean", C.c_float), ("mate_gap_stddev", C.c_float), ("read_length_mean", C.c_float),
                 ("seconds", C.c_double * STEP_COUNT), ("t_inflate", C.c_double), ("t_parse", C.c_double), ("t_finalize", C.c_double),
-                ("h2d_bytes", C.c_uint64), ("event_seconds", C.c_double * 32), ("output_seconds", C.c_double), ("n_candidates", C.c_uint64), ("n_unfiltered_candidates", C.c_uint64)]
+                ("h2d_bytes", C.c_uint64), ("event_seconds", C.c_double * 32), ("output_seconds", C.c_double), ("n_candidates", C.c_uint64), ("n_unfiltered_candidates", C.c_uint64),
+                ("chimeric_records", C.c_uint64), ("chimeric_malformed", C.c_uint64), ("chimeric_total", C.c_uint64)]
 
 
 def _load_pipeline_api(lib):
@@ -543,10 +544,12 @@ def _np_from(pointer, n, dtype):
 class Pipeline:
     """One run of the hot path on files: the call a user of the library makes (the `arriba` CLI is a thin wrapper over it).
 
-    `bam` is the alignment file: BAM, or SAM text (plain or BGZF-compressed), told apart by the content (DESIGN.md section 5)."""
+    `bam` is the alignment file: BAM, or SAM text (plain or BGZF-compressed), told apart by the content (DESIGN.md section 5). `chimeric` is STAR's
+    separate chimeric alignment file (Chimeric.out.sam, from --chimOutType SeparateSAMold; any of the same formats), read before `bam` (the -c option)."""
 
     def __init__(self, bam, gtf, fasta, threads=1, device=0, lib_path=None, strandedness=3, params=None, output=None, discarded=None,
-                 genomic_breakpoints=None, max_genomic_breakpoint_distance=100000, blacklist=None, known_fusions=None, tags=None, protein_domains=None):
+                 genomic_breakpoints=None, max_genomic_breakpoint_distance=100000, blacklist=None, known_fusions=None, tags=None, protein_domains=None,
+                 chimeric=None):
         self.lib = load(lib_path)
         _load_pipeline_api(self.lib)
         o = RunOptions()
@@ -568,6 +571,8 @@ class Pipeline:
             self._strings.append(tags.encode()); o.tags_file = self._strings[-1]
         if protein_domains:
             self._strings.append(protein_domains.encode()); o.protein_domains_file = self._strings[-1]
+        if chimeric:
+            self._strings.append(chimeric.encode()); o.chimeric_file = self._strings[-1]
         o.threads = threads; o.device = device; o.strandedness = strandedness
         if params is not None:
             o.params = params

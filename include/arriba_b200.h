@@ -124,7 +124,16 @@ int arb_push_chunk_end(arb_ctx* ctx, const arb_soa_chunk* chunk);
  *   arb_records_error_record : the record body (after block_size) an error of kinds 1-3 names,
  *   arb_records_finish : the replay; coverage / starts / ends = per contig caller-allocated windows (the counts of arb_records_begin), counters = mapped
  *                        reads, malformed supplementaries, secondaries without HI, 1 if any split read or discordant mate was seen, then the pristine reads
- *                        of every contig (4 + n_contigs); error as above. On success the fragment pools are ready for arb_fragment_table_build.
+ *                        of every contig (4 + n_contigs); error as above. On success the fragment pools are ready for arb_fragment_table_build. With an
+ *                        error the counters are those of the replay's counting pass (only the split-read flag of a -c file is meaningful).
+ * A separate chimeric file (-c Chimeric.out.sam, STAR --chimOutType SeparateSAMold; DESIGN.md section 5 has the rules) goes into the same store, ahead of
+ * the main file, and one replay runs both files' loops:
+ *   arb_records_source : after arb_records_begin, before a file's chunks (and, for SAM text, before its arb_records_text_names): chimeric_file != 0 for the
+ *                        -c file, 0 for the main file, which comes second; tid_to_contig maps this file's header (n_tid references).
+ *                        first_position = where this file's record positions start: the positions of errors (and of arb_records_text_chunk's staged
+ *                        records) continue behind the earlier file's, so an error at a position below the main file's first_position is the -c file's.
+ *                        Kind 5 is a -c record without a reference (its mapped-or-not state is not checked in that file). Without this call the chunks
+ *                        are the main file's, mapped by arb_records_begin's tid_to_contig, as before.
  * ---- fragment table from the pools ---------------------------------------------------------------------------------------------------------------
  * The pools: fragments (name, chain of alignments in the loop's order) and pools of names, CIGAR operations and nt16 sequences. The device turns them into
  * the resident fragment table: slot normalisation and rejection of malformed fragments (source/read_chimeric_alignments.cpp:340-506), name order
@@ -132,10 +141,13 @@ int arb_push_chunk_end(arb_ctx* ctx, const arb_soa_chunk* chunk);
  * slot 1) and the multimapper flags (:792-802).
  *   arb_fragment_table_build  : builds the table, which becomes the resident one (as after arb_push_chunk_begin); sizes = {fragments, rejected fragments,
  *                               CIGAR operations, sequence bytes, name bytes, neighbours in name order with the same read name (mark_multimappers' count)},
+ *   arb_fragment_table_chimeric_file : after arb_records_finish with a -c file (also one that reports an error): {-c fragments the first malformed pass
+ *                               rejects, -c fragments it keeps}, as the replay's counting pass decides them. The build's rejected fragments (sizes[1])
+ *                               include the first; the kept ones include the single-end -c fragments the build drops (the second pass rejects them),
  *   arb_fragment_table_download : the host copy (caller-allocated: n, n, n, 3n; 3n, 3n, 3n, 3n, 3n; 2n, 2n; 3n, 3n; CIGAR operations + 1, sequence bytes;
  *                               name bytes, n + 1 offsets). */
 typedef struct { uint8_t supplementary, first_in_pair, forward; uint16_t contig; int32_t start, end; uint32_t cigar_off, cigar_cnt; uint64_t seq_off; uint32_t seq_len; int32_t next; } arb_pool_alignment;
-typedef struct { uint64_t name_off; uint32_t name_len; int32_t head, tail; uint32_t count; uint8_t single_end, duplicate; } arb_pool_fragment;
+typedef struct { uint64_t name_off; uint32_t name_len; int32_t head, tail; uint32_t count; uint8_t single_end, duplicate, chimeric_file /* from the -c file */; } arb_pool_fragment;
 int arb_records_begin(arb_ctx* ctx, const uint16_t* tid_to_contig, uint32_t n_tid, const uint8_t* interesting, const uint8_t* viral, const uint64_t* n_windows, uint32_t n_contigs,
                       uint32_t max_itd_length, int external_duplicate_marking, uint64_t expected_bytes);
 int arb_records_chunk(arb_ctx* ctx, const uint8_t* chunk, uint64_t bytes, uint64_t first, uint64_t chunk_pos, uint64_t* n_records, uint64_t* carry, uint32_t* malformed, uint64_t* error);
@@ -148,10 +160,12 @@ int arb_records_finish(arb_ctx* ctx, uint16_t* const* coverage, uint8_t* const* 
  *                            The bytes after the last LF are kept for the next chunk (carry); with last != 0 they are the last line. error: as for
  *                            arb_records_chunk, with positions in the stream of staged records, which keeps file order; an unreadable line is an error of
  *                            kind 1. arb_records_error_record hands out the staged body. arb_records_finish follows as for BAM input. */
+int arb_records_source(arb_ctx* ctx, int chimeric_file, const uint16_t* tid_to_contig, uint32_t n_tid, uint64_t* first_position);
 int arb_records_text_names(arb_ctx* ctx, const char* names, const uint64_t* name_off, uint32_t n_names);
 int arb_records_text_chunk(arb_ctx* ctx, const uint8_t* chunk, uint64_t bytes, uint64_t first, uint64_t chunk_pos, int last, uint64_t* n_records, uint64_t* carry, uint64_t* error);
 int arb_fragment_table_build(arb_ctx* ctx, uint64_t sizes[6]);
 int arb_fragment_table_download(arb_ctx* ctx, const arb_soa_chunk* columns, char* names, uint64_t* name_off);
+int arb_fragment_table_chimeric_file(arb_ctx* ctx, uint64_t counts[2]);
 /* ---- annotation of the resident fragments -------------------------------------------------------------------
  * Replaces the annotation passes of main (source/arriba.cpp:165-325: annotate_alignments per fragment, source/annotation.cpp:431-555; dummy genes for
  * intergenic breakpoints, arriba.cpp:207-260; second pass :262-319) and assign_strands_from_strandedness (source/read_chimeric_alignments.cpp:775-790).
@@ -485,6 +499,7 @@ typedef struct arb_run_options {
 	const char* known_fusions_file;  /* -k: known fusions (optionally .gz), NULL = none; read only while the known_fusions filter is on */
 	const char* tags_file;           /* -t: tags (optionally .gz), NULL = none */
 	const char* protein_domains_file; /* -p: protein domains (GFF3, optionally .gz), NULL = none */
+	const char* chimeric_file;       /* -c: STAR's Chimeric.out.sam (SAM, BGZF SAM or BAM; --chimOutType SeparateSAMold), NULL = none */
 } arb_run_options;
 void arb_default_run_options(arb_run_options* o);
 
@@ -501,6 +516,8 @@ typedef struct arb_run_stats {
 	double event_seconds[32];            /* wall time per event-level stage (ARB_EV_*) */
 	double output_seconds;               /* arb_pipeline_write_output */
 	uint64_t n_candidates, n_unfiltered_candidates;
+	/* the -c file (zero without one): its records, the fragments the first malformed pass rejected, and those it kept (its progress line's total) */
+	uint64_t chimeric_records, chimeric_malformed, chimeric_total;
 } arb_run_stats;
 
 int arb_pipeline_create(arb_pipeline** out, const arb_run_options* options);

@@ -8,8 +8,11 @@ Also the rate of a plain copy of one page-locked 128 MiB host buffer to the devi
 With --sam (or --sam-bgzf) the SAM text rendering of the same world (tools/synth.cpp --sam-only, written once next to the BAM) is measured too: BAM and SAM
 steps alternate, after one warm-up of each, and every format gets its own medians, its input size and the SAM parse lap (rec_text_parse_ms, part of
 rec_chunk_kernels_ms).
+With --separate-chimeric the world is also written as STAR's --chimOutType SeparateSAMold pair (tools/synth.cpp --separate-chimeric-only: the chimeric
+reads in Chimeric.out.sam, SAM text, the rest in Aligned.out.bam), and the pair (-c and -x) is timed against the WithinBAM file, alternating; the pair's
+input_bytes is the main file's, chimeric_input_bytes the -c file's.
 
-python tools/ingest_bench.py [--warmup 1] [--steps 3] [--threads N] [--sam | --sam-bgzf]"""
+python tools/ingest_bench.py [--warmup 1] [--steps 3] [--threads N] [--sam | --sam-bgzf | --separate-chimeric]"""
 import argparse, json, os, statistics, subprocess, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -33,8 +36,8 @@ def pinned_h2d_gbps(reps=10):
     return reps * (128 << 20) / (a.elapsed_time(b) * 1e-3) / 1e9
 
 
-def one_step(prefix, threads, path=None):
-    p = L.Pipeline(path or prefix + ".bam", prefix + ".gtf", prefix + ".fa", threads=threads)
+def one_step(prefix, threads, path=None, chimeric=None):
+    p = L.Pipeline(path or prefix + ".bam", prefix + ".gtf", prefix + ".fa", threads=threads, chimeric=chimeric)
     p.step(L.STEP_LOAD_REFERENCE)
     t0 = time.perf_counter()
     p.step(L.STEP_INGEST)
@@ -45,6 +48,8 @@ def one_step(prefix, threads, path=None):
     r = {"ingest_s": round(ingest_s, 3), "ingest_split": {"inflate": round(s.t_inflate, 3), "parse": round(s.t_parse, 3), "finalize": round(s.t_finalize, 3)},
          "bam_scan_ms": round(t.bam_scan_ms, 1), "laps_ms": laps, "finalize_rest_s": round(s.t_finalize - finish_ms * 1e-3, 3),
          "records": int(s.n_records), "fragments": int(s.n_fragments)}
+    if chimeric:
+        r.update(chimeric_records=int(s.chimeric_records), chimeric_total=int(s.chimeric_total), chimeric_malformed=int(s.chimeric_malformed))
     p.close()
     return r
 
@@ -56,12 +61,13 @@ def main():
     ap.add_argument("--workload", default="cfg2_10M_2x101_50k")
     ap.add_argument("--sam", action="store_true", help="also the plain SAM rendering of the world")
     ap.add_argument("--sam-bgzf", action="store_true", help="also the BGZF-compressed SAM rendering (level 1)")
+    ap.add_argument("--separate-chimeric", action="store_true", help="also the SeparateSAMold pair (-c Chimeric.out.sam -x Aligned.out.bam)")
     a = ap.parse_args()
     if not os.path.exists(_build.PRODUCT_LIB):
         _build.build_product()
     prefix = bench.ensure_world(a.workload)
     card = bench.ClockSampler(0).card()
-    inputs = {"bam": prefix + ".bam"}
+    inputs = {"bam": (prefix + ".bam", None)}
     if a.sam or a.sam_bgzf:
         kind = "sam_bgzf" if a.sam_bgzf else "sam"
         sam_prefix = prefix + "_" + kind
@@ -70,18 +76,27 @@ def main():
                 os.symlink(prefix + ".bam", sam_prefix + ".bam")
             subprocess.run([_build.build_tools(), "--prefix", sam_prefix, "--sam-only"] + (["--sam-bgzf", "1"] if a.sam_bgzf else []), check=True)
             open(sam_prefix + ".done", "w").write("ok")
-        inputs[kind] = sam_prefix + ".sam"
+        inputs[kind] = (sam_prefix + ".sam", None)
+    if a.separate_chimeric:
+        pair_prefix = prefix + "_separate"
+        if not os.path.exists(pair_prefix + ".done"):
+            if not os.path.exists(pair_prefix + ".bam"):
+                os.symlink(prefix + ".bam", pair_prefix + ".bam")
+            subprocess.run([_build.build_tools(), "--prefix", pair_prefix, "--separate-chimeric-only"], check=True)
+            open(pair_prefix + ".done", "w").write("ok")
+        inputs["separate_chimeric"] = (pair_prefix + ".Aligned.out.bam", pair_prefix + ".Chimeric.out.sam")
     for _ in range(a.warmup):
-        for path in inputs.values():
-            one_step(prefix, a.threads, path)
+        for path, chimeric in inputs.values():
+            one_step(prefix, a.threads, path, chimeric)
     steps = {k: [] for k in inputs}
     for _ in range(a.steps):  # the formats alternate
-        for k, path in inputs.items():
-            steps[k].append(one_step(prefix, a.threads, path))
+        for k, (path, chimeric) in inputs.items():
+            steps[k].append(one_step(prefix, a.threads, path, chimeric))
     out = {"workload": a.workload, "threads": a.threads, **card, "pinned_h2d_128MiB_GBps": round(pinned_h2d_gbps(), 2)}
     for k, st in steps.items():
         med = lambda f: statistics.median(f(r) for r in st)
-        out[k] = {"input_bytes": os.path.getsize(inputs[k]),
+        path, chimeric = inputs[k]
+        out[k] = {"input_bytes": os.path.getsize(path), **({"chimeric_input_bytes": os.path.getsize(chimeric)} if chimeric else {}),
                   "median": {"ingest_s": med(lambda r: r["ingest_s"]), "finalize_s": med(lambda r: r["ingest_split"]["finalize"]), "bam_scan_ms": med(lambda r: r["bam_scan_ms"]),
                              "laps_ms": {x: med(lambda r: r["laps_ms"][x]) for x in LAPS}},
                   "steps": st}

@@ -15,6 +15,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <unordered_set>
 #include <vector>
 
 using namespace std;
@@ -914,19 +915,101 @@ static void write_sam(const string& bam_path, const string& sam_path, int bgzf_l
 	if (plain) fclose(plain); else z.close();
 }
 
+// ---------------------------------------------------------------------------------- the same records as STAR's --chimOutType SeparateSAMold pair
+// A read's records under one key (name and HI) are chimeric when one of them is supplementary (0x800), a discordant mate or carries an SA tag. The chimeric
+// records of keys with HI 1 go to <out>.Chimeric.out.sam (SAM text, as STAR writes it) with 0x800 turned into 0x100 and without their HI and SA tags; every
+// other record goes to <out>.Aligned.out.bam, unchanged (BGZF at `level`). Both files carry the BAM's header.
+static void write_separate_chimeric(const string& bam_path, const string& out, int level) {
+	auto open_in = [&]() { gzFile in = gzopen(bam_path.c_str(), "rb"); if (!in) { perror(bam_path.c_str()); exit(1); } return in; };
+	struct record_t { vector<unsigned char> b; string key; bool chimeric; int hit; };
+	// every record as (body, "<qname>,<HI>", chimeric on its own, HI)
+	auto each = [&](gzFile in, string& header_raw, vector<string>& names, vector<uint32_t>& lengths, auto f) {
+		auto need = [&](void* p, unsigned n) { if (gzread(in, p, n) != (int) n) { fprintf(stderr, "synth: truncated BAM %s\n", bam_path.c_str()); exit(1); } };
+		auto rd32 = [&]() { uint32_t v; need(&v, 4); return v; };
+		char magic[4]; need(magic, 4);
+		string text(rd32(), '\0'); if (!text.empty()) need(&text[0], text.size());
+		header_raw.assign(magic, 4); uint32_t l = (uint32_t) text.size(); header_raw.append((const char*) &l, 4); header_raw += text;
+		const uint32_t n_ref = rd32(); header_raw.append((const char*) &n_ref, 4);
+		names.assign(n_ref, string()); lengths.assign(n_ref, 0);
+		for (uint32_t k = 0; k < n_ref; ++k) {
+			const uint32_t ln = rd32(); string n(ln, '\0'); need(&n[0], ln); const uint32_t len = rd32();
+			header_raw.append((const char*) &ln, 4); header_raw += n; header_raw.append((const char*) &len, 4); names[k] = n.c_str(); lengths[k] = len;
+		}
+		record_t r; uint32_t bs;
+		while (gzread(in, &bs, 4) == 4) {
+			r.b.resize(bs); need(r.b.data(), bs);
+			const unsigned char* b = r.b.data();
+			uint32_t flag = (uint32_t) b[14] | (uint32_t) b[15] << 8, nc = (uint32_t) b[12] | (uint32_t) b[13] << 8, ls; memcpy(&ls, b + 16, 4);
+			size_t at = 32 + b[8] + 4 * (size_t) nc + (ls + 1) / 2 + ls;
+			bool sa = false; r.hit = 1;
+			while (at + 3 <= bs) { // the tags synth writes: C (integers) and Z
+				if (b[at] == 'S' && b[at + 1] == 'A') sa = true;
+				if (b[at + 2] == 'C') { if (b[at] == 'H' && b[at + 1] == 'I') r.hit = b[at + 3]; at += 4; }
+				else { at += 3; while (at < bs && b[at]) ++at; ++at; }
+			}
+			r.key = string((const char*) b + 32) + "," + to_string(r.hit);
+			r.chimeric = (flag & 2048) || ((flag & 1) && !(flag & 2)) || sa;
+			f(r);
+		}
+	};
+	string header_raw; vector<string> names; vector<uint32_t> lengths;
+	unordered_set<string> chimeric;
+	{ gzFile in = open_in(); each(in, header_raw, names, lengths, [&](const record_t& r) { if (r.chimeric && r.hit == 1) chimeric.insert(r.key); }); gzclose(in); }
+	bam_writer_t x; x.open(out + ".Aligned.out.bam", level); x.write(header_raw.data(), header_raw.size());
+	FILE* c = fopen((out + ".Chimeric.out.sam").c_str(), "wb"); if (!c) { perror(out.c_str()); exit(1); }
+	for (size_t k = 0; k < names.size(); ++k) fprintf(c, "@SQ\tSN:%s\tLN:%u\n", names[k].c_str(), lengths[k]);
+	static const char ops[] = "MIDNSHP=X", bases[] = "=ACMGRSVTWYHKDBN";
+	string line;
+	gzFile in = open_in();
+	each(in, header_raw, names, lengths, [&](const record_t& r) {
+		if (!chimeric.count(r.key)) { const uint32_t bs = (uint32_t) r.b.size(); x.write(&bs, 4); x.write(r.b.data(), bs); return; }
+		const unsigned char* b = r.b.data(); const size_t bs = r.b.size();
+		auto u32 = [&](size_t at) { uint32_t v; memcpy(&v, b + at, 4); return v; };
+		const int32_t tid = (int32_t) u32(0), pos = (int32_t) u32(4), mtid = (int32_t) u32(20), mpos = (int32_t) u32(24), tlen = (int32_t) u32(28);
+		uint32_t flag = (uint32_t) b[14] | (uint32_t) b[15] << 8; const uint32_t nc = (uint32_t) b[12] | (uint32_t) b[13] << 8, ls = u32(16);
+		if (flag & 2048) flag = (flag & ~2048u) | 256u;
+		size_t at = 32;
+		line.assign((const char*) b + at); at += b[8];
+		line += "\t" + to_string(flag) + "\t" + (tid < 0 ? string("*") : names[tid]) + "\t" + to_string(pos + 1) + "\t" + to_string(b[9]) + "\t";
+		for (uint32_t k = 0; k < nc; ++k) { const uint32_t op = u32(at + 4 * k); line += to_string(op >> 4); line += ops[op & 15]; }
+		if (nc == 0) line += "*";
+		at += 4 * nc;
+		line += "\t" + (mtid < 0 ? string("*") : mtid == tid ? string("=") : names[mtid]) + "\t" + to_string(mpos + 1) + "\t" + to_string(tlen) + "\t";
+		for (uint32_t i = 0; i < ls; ++i) line += bases[(b[at + i / 2] >> (i & 1 ? 0 : 4)) & 15];
+		if (ls == 0) line += "*";
+		at += (ls + 1) / 2;
+		line += "\t";
+		for (uint32_t i = 0; i < ls; ++i) line += (char) (b[at + i] + 33);
+		if (ls == 0) line += "*";
+		at += ls;
+		while (at + 3 <= bs) {
+			const bool drop = (b[at] == 'H' && b[at + 1] == 'I') || (b[at] == 'S' && b[at + 1] == 'A');
+			string field; field += (char) b[at]; field += (char) b[at + 1];
+			if (b[at + 2] == 'C') { field += ":i:" + to_string(b[at + 3]); at += 4; }
+			else { const string v((const char*) b + at + 3); field += ":Z:" + v; at += 3 + v.size() + 1; }
+			if (!drop) line += "\t" + field;
+		}
+		line += "\n";
+		fwrite(line.data(), 1, line.size(), c);
+	});
+	gzclose(in); fclose(c); x.close();
+}
+
 static void usage() {
 	fprintf(stderr,
 		"usage: synth --prefix P [--seed S] [--scale F] [--genes G] [--breakpoints B] [--fragments N] [--read-length L]\n"
 		"             [--normal-frac F] [--split-frac F] [--dup-frac F] [--multimap-frac F] [--mismapper-frac F] [--paralog-frac F]\n"
 		"             [--deep-frac F] [--deep-depth D] [--shuffle] [--varnames] [--compress LEVEL] [--chr] [--reads-only]\n"
-		"             [--sam] [--sam-bgzf LEVEL] [--sam-only]\n"
-		"  --sam: also write P.sam, the records of P.bam as SAM text (--sam-bgzf: BGZF-compressed at LEVEL); --sam-only: convert an existing P.bam\n");
+		"             [--sam] [--sam-bgzf LEVEL] [--sam-only] [--separate-chimeric] [--separate-chimeric-only]\n"
+		"  --sam: also write P.sam, the records of P.bam as SAM text (--sam-bgzf: BGZF-compressed at LEVEL); --sam-only: convert an existing P.bam\n"
+		"  --separate-chimeric: also write P.bam as STAR's --chimOutType SeparateSAMold pair, P.Chimeric.out.sam and P.Aligned.out.bam;\n"
+		"                       --separate-chimeric-only: convert an existing P.bam\n");
 	exit(1);
 }
 
 int main(int argc, char** argv) {
 	params_t P;
-	bool sam = false, sam_only = false; int sam_level = -1;
+	bool sam = false, sam_only = false, separate = false, separate_only = false; int sam_level = -1;
 	for (int i = 1; i < argc; ++i) {
 		string a = argv[i];
 		#define NEXT (i + 1 < argc ? argv[++i] : (usage(), (char*) NULL))
@@ -957,9 +1040,15 @@ int main(int argc, char** argv) {
 		else if (a == "--sam") sam = true;
 		else if (a == "--sam-bgzf") { sam = true; sam_level = atoi(NEXT); }
 		else if (a == "--sam-only") { sam = true; sam_only = true; }
+		else if (a == "--separate-chimeric") separate = true;
+		else if (a == "--separate-chimeric-only") { separate = true; separate_only = true; }
 		else usage();
 	}
-	if (sam_only) { write_sam(P.prefix + ".bam", P.prefix + ".sam", sam_level); return 0; }
+	if (sam_only || separate_only) {
+		if (sam_only) write_sam(P.prefix + ".bam", P.prefix + ".sam", sam_level);
+		if (separate_only) write_separate_chimeric(P.prefix + ".bam", P.prefix, P.compress);
+		return 0;
+	}
 	rng_t rng(P.seed);
 	world_t w;
 	make_genome(w, P, rng);
@@ -972,6 +1061,7 @@ int main(int argc, char** argv) {
 	generator_t gen(w, P);
 	gen.run(P.prefix + ".bam");
 	if (sam) write_sam(P.prefix + ".bam", P.prefix + ".sam", sam_level);
+	if (separate) write_separate_chimeric(P.prefix + ".bam", P.prefix, P.compress);
 	size_t total = 0; for (size_t c = 0; c < w.seq.size(); ++c) total += w.seq[c].size();
 	fprintf(stderr, "synth: genome=%zu bp, genes=%zu, breakpoints=%zu, chimeric fragments=%ld\n", total, w.genes.size(), w.bps.size(), gen.n_emitted_fragments);
 	return 0;
