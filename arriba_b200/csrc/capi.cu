@@ -227,6 +227,14 @@ int arb_retained_protein_domains(arb_ctx* ctx, uint32_t n_ids, const uint32_t* i
 	ARB_API_BEGIN(ctx) const uint64_t b = ctx->e.retained_protein_domains(n_ids, ids); if (n_bytes) *n_bytes = b; ARB_API_END(ctx)
 }
 int arb_get_retained_protein_domains(arb_ctx* ctx, uint64_t* off, char* text) { ARB_API_BEGIN(ctx) ctx->e.get_retained_protein_domains(off, text); ARB_API_END(ctx) }
+int arb_set_fill_transcripts(arb_ctx* ctx, uint32_t n, const int32_t* first_exon, const int32_t* last_exon, const uint32_t* contig, const int32_t* exon_next, const int32_t* exon_prev) {
+	ARB_API_BEGIN(ctx) ctx->e.set_fill_transcripts(n, first_exon, last_exon, contig, exon_next, exon_prev); ARB_API_END(ctx)
+}
+int arb_fill_gaps(arb_ctx* ctx, uint32_t n_rows, const char* text, const uint32_t* row_off, const int32_t* pos, const uint32_t* pos_off, uint32_t n_jobs, const uint32_t* row, const uint32_t* transcript,
+                  const uint8_t* flags, uint64_t* n_chars) {
+	ARB_API_BEGIN(ctx) const uint64_t n = ctx->e.fill_gaps(n_rows, text, row_off, pos, pos_off, n_jobs, row, transcript, flags); if (n_chars) *n_chars = n; ARB_API_END(ctx)
+}
+int arb_get_filled(arb_ctx* ctx, uint32_t* off, char* chars, int32_t* pos) { ARB_API_BEGIN(ctx) ctx->e.get_filled(off, chars, pos); ARB_API_END(ctx) }
 int arb_get_slot_swaps(arb_ctx* ctx, uint8_t* out) { ARB_API_BEGIN(ctx) ctx->e.get_slot_swaps(out); ARB_API_END(ctx) }
 
 } // extern "C"

@@ -218,6 +218,12 @@ public:
 	struct domain_view domain_tables(); void check_domain_error(const char* who);
 	dbuf<u16> dom_contig; dbuf<i32> dom_start, dom_end; dbuf<u32> dom_mult, dom_name, dom_gene_off, dom_name_off, dom_error; dbuf<char> dom_name_chars, dom_text;
 	std::vector<u64> dom_text_off; u32 dom_records; bool has_protein_domains;
+	// gap filling of fusion transcript sequences (-I, fill_gaps.cu): the transcript table of the writer, and the filled sides of the last call
+	void set_fill_transcripts(u32 n, const i32* first_exon, const i32* last_exon, const u32* contig, const i32* exon_next, const i32* exon_prev);
+	u64 fill_gaps(u32 n_rows, const char* text, const u32* row_off, const i32* pos, const u32* pos_off, u32 n_jobs, const u32* row, const u32* transcript, const u8* flags);
+	void get_filled(u32* off, char* chars, i32* pos);
+	dbuf<i32> fill_first, fill_last, fill_next, fill_prev, fill_pos; dbuf<u32> fill_contig; dbuf<char> fill_chars; std::vector<u32> fill_off;
+	u32 fill_transcript_count = 0; u64 fill_chars_total = 0; bool has_fill_transcripts = false;
 private:
 	read_filter_params make_filter_params();
 	unsigned long genome_size() const;

@@ -1,6 +1,6 @@
 // cli_main.cpp -- the `arriba` command line of arriba-b200: same option letters, defaults and error texts as the reference
 // (options.cpp:270-485, usage options.cpp:109-268), driving the pipeline through the public C ABI only.
-// Not supported (fail loudly): -G, -I.
+// Not supported (fail loudly): -G.
 #include <getopt.h>
 #include <unistd.h>
 #include <sys/resource.h>
@@ -45,7 +45,8 @@ static void usage() {
 	          << " -k FILE  known fusions (optionally .gz)   -t FILE  tags (optionally .gz)\n"
 	          << " -p FILE  protein domains (GFF3, optionally .gz)\n"
 	          << " -d FILE  genomic breakpoints from whole-genome sequencing (four-column or VCF, optionally .gz)\n -D N     maximum genomic breakpoint distance (default 100000)\n"
-	          << " -@ N     host threads for decoding and annotation   -u external duplicate marking   -X extra info for discarded candidates\n";
+	          << " -@ N     host threads for decoding and annotation   -u external duplicate marking   -X extra info for discarded candidates\n"
+	          << " -I       fill gaps in the fusion_transcript column with the exons of the chosen transcripts (in the discarded file only with -X)\n";
 }
 
 int main(int argc, char** argv) {
@@ -81,7 +82,8 @@ int main(int argc, char** argv) {
 					std::cerr << "WARNING: it seems you passed the chimeric junction file ('Chimeric.out.junction') to the parameter -c, but this parameter takes the chimeric alignments file ('Chimeric.out.sam') as input" << std::endl;
 				break;
 			}
-			case 'G': case 'I':
+			case 'I': o.fill_sequence_gaps = 1; break;
+			case 'G':
 				crash(true, "option " + opt + " is not supported by arriba-b200 (see DESIGN.md, out of scope)"); break;
 			case 's': { const std::string m = optarg; o.strandedness = m == "auto" ? 3 : m == "yes" ? 1 : m == "no" ? 0 : m == "reverse" ? 2 : -1; crash(o.strandedness < 0, "invalid type of strandedness: " + m); break; }
 			case 'i': interesting = optarg; std::replace(interesting.begin(), interesting.end(), ',', ' '); break;

@@ -67,6 +67,7 @@ int arb_pipeline_create(arb_pipeline** out, const arb_run_options* o) {
 		if (o->tags_file) r.tags_file = o->tags_file;
 		if (o->protein_domains_file) r.protein_domains_file = o->protein_domains_file;
 		if (o->chimeric_file) r.chimeric_file = o->chimeric_file;
+		r.fill_sequence_gaps = o->fill_sequence_gaps != 0;
 		r.params = o->params; r.strandedness = o->strandedness; r.fragment_length = o->fragment_length; r.threads = o->threads; r.device = o->device;
 		*out = x;
 	} catch (const std::exception& e) { g_pipeline_create_error = e.what(); return 1; }

@@ -1,5 +1,5 @@
 // output.cpp -- writer of fusions.tsv / fusions.discarded.tsv.
-// Behavioural contract: write_fusions_to_file and helpers (output_fusions.cpp:25-1261, without the optional gap filling -I),
+// Behavioural contract: write_fusions_to_file and helpers (output_fusions.cpp:25-1261; the gap filling of -I on the device, fill_gaps_hd.h),
 // get_fusion_peptide_sequence / is_in_frame / get_reading_frame / translate_reference_protein (annotate_protein_domains.cpp:164-446).
 // Tags (-t) and protein domains (-p) need database files that are not part of the reference repository; their columns are ".".
 #include "pipeline.h"
@@ -15,6 +15,7 @@
 #include <chrono>
 #include <cmath>
 #include <cstring>
+#include <deque>
 #include <fstream>
 #include <iostream>
 #include <map>
@@ -687,9 +688,42 @@ struct writer {
 		return ref.original_names[contig] + ":" + std::to_string((long long) (genomic + 1)) + "(" + std::to_string((long long) std::abs(bp - genomic)) + ")";
 	}
 
+	// -I: the filled sides of one row (fill_gaps_hd.h), P5 per 5' transcript and S3 per 3' transcript, in a block of the writer's
+	struct filled_row {
+		struct half { i32 transcript; bool three; u32 off, len; };
+		std::vector<half> halves; const std::string* chars; const std::vector<i32>* pos;
+		filled_row(): chars(NULL), pos(NULL) {}
+		const half* find(i32 t, bool three) const { for (size_t h = 0; h < halves.size(); ++h) if (halves[h].transcript == t && halves[h].three == three) return &halves[h]; return NULL; }
+		// the sequence of the pair (t5, t3): P5 + seq[b5 .. b3] + S3 (a side without a transcript, -1, stays as it is)
+		void assemble(i32 t5, i32 t3, const std::string& seq, const std::vector<i32>& positions, std::string& s, std::vector<i32>& p) const {
+			s = seq; p = positions;
+			const size_t b5 = seq.find('|'), b3 = seq.rfind('|');
+			if (b5 >= seq.size()) return; // no transcripts: nothing to fill
+			const half* h5 = t5 >= 0 ? find(t5, false) : NULL; const half* h3 = t3 >= 0 ? find(t3, true) : NULL;
+			s.clear(); p.clear();
+			if (h5) { s.append(*chars, h5->off, h5->len); p.insert(p.end(), pos->begin() + h5->off, pos->begin() + h5->off + h5->len); }
+			else { s.append(seq, 0, b5); p.insert(p.end(), positions.begin(), positions.begin() + b5); }
+			s.append(seq, b5, b3 - b5 + 1); p.insert(p.end(), positions.begin() + b5, positions.begin() + b3 + 1);
+			if (h3) { s.append(*chars, h3->off, h3->len); p.insert(p.end(), pos->begin() + h3->off, pos->begin() + h3->off + h3->len); }
+			else { s.append(seq, b3 + 1, std::string::npos); p.insert(p.end(), positions.begin() + b3 + 1, positions.end()); }
+		}
+	};
+	// the unfilled transcript sequence of a row and the transcripts that match its two sides (output_fusions.cpp:1133-1141)
+	struct row_transcripts { std::string tseq; std::vector<i32> positions, t5, t3; };
+	void transcripts_of_row(u32 k, const side_strings* from_device, row_transcripts& r) const {
+		u32 g5 = e.gene1[k], g3 = e.gene2[k]; bool st5 = e.bits[k] & CB_PSTRAND1, st3 = e.bits[k] & CB_PSTRAND2;
+		if (!(e.bits[k] & CB_TSTART_GENE1)) { std::swap(g5, g3); std::swap(st5, st3); }
+		const bool ambiguous = e.bits[k] & CB_PSTRANDS_AMBIGUOUS;
+		r.tseq = ".";
+		transcript_sequence(k, r.tseq, r.positions, from_device);
+		matching_transcripts(r.tseq, r.positions, g5, st5, ambiguous, 5, r.t5);
+		matching_transcripts(r.tseq, r.positions, g3, st3, ambiguous, 3, r.t3);
+	}
+	bool is_itd(u32 k) const { return e.gene1[k] == e.gene2[k] && ((unsigned int) e.bp2[k] - (unsigned int) e.bp1[k]) < p.opt.params.max_itd_length && e.dir1[k] == UPSTREAM && e.dir2[k] == DOWNSTREAM; }
+
 	// a row with the columns of -X (fusion transcript, peptide, reading frame, read names): every row formatted on the host has them (the discarded file
-	// without -X is formatted on the device, format_discarded_rows_on_device)
-	void format_row(row_buffer& out, u32 k, const side_strings* from_device = NULL) const {
+	// without -X is formatted on the device, format_discarded_rows_on_device). With -I, `pre` holds the row's transcripts and `fill` its filled sides.
+	void format_row(row_buffer& out, u32 k, const side_strings* from_device = NULL, row_transcripts* pre = NULL, const filled_row* fill = NULL) const {
 			static const char* CONF[] = {"low", "medium", "high", "high"};
 			std::string site5 = site(e.gene1[k], e.spliced1(k), e.exonic1(k), e.contig1[k], e.bp1[k]), site3 = site(e.gene2[k], e.spliced2(k), e.exonic2(k), e.contig2[k], e.bp2[k]);
 			u32 g5 = e.gene1[k], g3 = e.gene2[k], c5 = e.contig1[k], c3 = e.contig2[k], d5 = e.dir1[k], d3 = e.dir2[k], s5 = e.split_reads1[k], s3 = e.split_reads2[k];
@@ -698,22 +732,25 @@ struct writer {
 			const bool ambiguous = e.bits[k] & CB_PSTRANDS_AMBIGUOUS;
 			if (!(e.bits[k] & CB_TSTART_GENE1)) { std::swap(g5, g3); std::swap(c5, c3); std::swap(d5, d3); std::swap(s5, s3); std::swap(b5, b3); std::swap(st5, st3); std::swap(site5, site3); std::swap(gb5, gb3); }
 			const int cov5 = p.coverage.get_coverage(c5, b5, d5 == UPSTREAM ? DOWNSTREAM : UPSTREAM), cov3 = p.coverage.get_coverage(c3, b3, d3 == UPSTREAM ? DOWNSTREAM : UPSTREAM);
-			std::string tseq = ".", pep = ".", frame = "."; i32 tr5 = -1, tr3 = -1;
-			std::vector<i32> positions;
-			transcript_sequence(k, tseq, positions, from_device);
-			std::vector<i32> t5, t3;
-			matching_transcripts(tseq, positions, g5, st5, ambiguous, 5, t5);
-			matching_transcripts(tseq, positions, g3, st3, ambiguous, 3, t3);
+			std::string pep = ".", frame = "."; i32 tr5 = -1, tr3 = -1;
+			row_transcripts own;
+			row_transcripts& rt = pre ? *pre : own;
+			if (!pre) transcripts_of_row(k, from_device, rt);
+			std::string& tseq = rt.tseq; const std::vector<i32>& positions = rt.positions; const std::vector<i32>& t5 = rt.t5; const std::vector<i32>& t3 = rt.t3;
+			std::string filled; std::vector<i32> filled_positions;
 			for (size_t i = 0; (t5.empty() || i < t5.size()) && frame != "in-frame"; ++i) { // try transcript pairs until one is in-frame
 				if (i < t5.size()) tr5 = t5[i];
 				for (size_t j = 0; (t3.empty() || j < t3.size()) && frame != "in-frame"; ++j) {
 					if (j < t3.size()) tr3 = t3[j];
-					pep = peptide(tseq, positions, g5, g3, tr5, tr3, st3); frame = frame_label(pep);
+					if (fill) { fill->assemble(tr5, tr3, tseq, positions, filled, filled_positions); pep = peptide(filled, filled_positions, g5, g3, tr5, tr3, st3); }
+					else pep = peptide(tseq, positions, g5, g3, tr5, tr3, st3);
+					frame = frame_label(pep);
 					if (j >= t3.size()) break;
 				}
 				if (i >= t5.size() || t3.empty()) break;
 			}
 			if (frame == "stop-codon") pep = ".";
+			if (fill) tseq.swap(filled); // the sequence of the last pair tried
 			out << gene_name(g5, c5, b5) << "\t" << gene_name(g3, c3, b3) << "\t" << strand_column(st5, g5, ambiguous) << "\t" << strand_column(st3, g3, ambiguous) << "\t"
 			    << ref.original_names[c5] << ":" << (b5 + 1) << "\t" << ref.original_names[c3] << ":" << (b3 + 1) << "\t" << site5 << "\t" << site3 << "\t"
 			    << fusion_type(k) << "\t" << s5 << "\t" << s3 << "\t" << e.discordant_mates[k] << "\t"
@@ -857,6 +894,7 @@ struct writer {
 		const std::string header = header_line();
 		device_consensus from_device;
 		if (!discarded && (getenv("ARB_DEVICE_CONSENSUS") == NULL || atoi(getenv("ARB_DEVICE_CONSENSUS")) != 0)) { consensus_on_device(rows, from_device); laps.lap(which, "pileups + consensus (device)"); }
+		if (p.opt.fill_sequence_gaps) { out.header = header; format_filled_rows(rows, from_device, out, which); return; }
 		// Rows are independent and cost very different amounts (the best-supported fusions come first and carry hundreds of reads each): threads draw small
 		// chunks of rows from a shared counter; every chunk is formatted into its own string and later copied to its offset of the file (flush_rows).
 		const size_t CHUNK = 32;
@@ -890,6 +928,115 @@ struct writer {
 			for (size_t t = 0; t < pool.size(); ++t) pool[t].join();
 		}
 		for (int t = 0; t < T; ++t) if (!errors[t].empty()) throw std::runtime_error(errors[t]);
+		laps.lap(which, "rows formatted");
+	}
+	// -I: the rows in blocks of ROW_BLOCK; per block (A) the transcript sequences and matching transcripts of the rows on the host threads, (B) every
+	// distinct (row, side, transcript) job filled on the device (fill_gaps_hd.h), in calls of at most FILL_CHARS output characters, (C) the transcript pairs
+	// of every row tried in the reference's order on the host threads and the rows formatted. Warnings stay with the chunk of rows that printed them (C).
+	enum { ROW_BLOCK = 32 * 1024, FILL_CHARS = 32 << 20 };
+	template <class F> void for_chunks(size_t lo, size_t hi, size_t chunk, F fn) const { // chunks [lo, hi) of `chunk` rows drawn by the host threads
+		const size_t n_chunks = (hi - lo + chunk - 1) / chunk;
+		const int T = std::max(1, std::min(p.threads, (int) (n_chunks ? n_chunks : 1)));
+		std::vector<std::string> errors(T); std::atomic<size_t> next_chunk(0); std::vector<std::thread> pool;
+		for (int t = 0; t < T; ++t) pool.emplace_back([&, t]() {
+			try { for (;;) { const size_t c = next_chunk.fetch_add(1); if (c >= n_chunks) break; fn(lo / chunk + c, lo + c * chunk, std::min(hi, lo + (c + 1) * chunk)); } }
+			catch (const std::exception& ex) { errors[t] = ex.what(); }
+			warning_sink = NULL;
+		});
+		for (size_t t = 0; t < pool.size(); ++t) pool[t].join();
+		for (int t = 0; t < T; ++t) if (!errors[t].empty()) throw std::runtime_error(errors[t]);
+	}
+	void upload_fill_transcripts() const {
+		pipeline& pl = p;
+		if (pl.fill_transcripts_on_device) return;
+		const size_t n = ref.transcripts.size(), E = ref.exons.size();
+		std::vector<i32> first(n ? n : 1, 0), last(n ? n : 1, 0), next(E ? E : 1, -1), prev(E ? E : 1, -1); std::vector<u32> contig(n ? n : 1, 0);
+		for (size_t t = 0; t < n; ++t) {
+			const transcript_rec& T = ref.transcripts[t];
+			if (T.first_exon < 0 || T.last_exon < 0) continue; // a transcript without exons matches no row (matching_transcripts finds transcripts by their exons)
+			first[t] = T.first_exon; last[t] = T.last_exon; contig[t] = ref.genes[ref.exons[T.first_exon].gene].contig;
+		}
+		for (size_t x = 0; x < E; ++x) { next[x] = ref.exons[x].next >= 0 ? ref.exons[x].next : -1; prev[x] = ref.exons[x].prev >= 0 ? ref.exons[x].prev : -1; }
+		if (arb_set_fill_transcripts(pl.ctx, (u32) n, first.data(), last.data(), contig.data(), next.data(), prev.data()) != 0) throw std::runtime_error(std::string("arb_set_fill_transcripts: ") + arb_last_error(pl.ctx));
+		pl.fill_transcripts_on_device = true;
+	}
+	// an upper bound of the characters a job writes: its side of the sequence, and every exon of the transcript with its "___" and the marks
+	u64 fill_bound(i32 t, size_t side) const {
+		u64 b = side + 8;
+		for (i32 ex = ref.transcripts[t].first_exon; ex >= 0; ex = ref.exons[ex].next >= 0 ? ref.exons[ex].next : -1) b += (u64) std::max(0, ref.exons[ex].end - ref.exons[ex].start + 1) + 3;
+		return b;
+	}
+	void format_filled_rows(const std::vector<u32>& rows, const device_consensus& from_device, formatted& out, const char* which) const {
+		output_laps laps;
+		upload_fill_transcripts();
+		pipeline& pl = p;
+		const size_t CHUNK = 32, n_chunks = (rows.size() + CHUNK - 1) / CHUNK;
+		out.slices.assign(n_chunks, std::string()); out.warnings.assign(n_chunks, std::string());
+		std::vector<row_transcripts> pre; std::vector<filled_row> fill;
+		std::deque<std::string> block_chars; std::deque<std::vector<i32> > block_pos; // the outputs of the calls of a block (a deque keeps them in place)
+		u64 n_jobs = 0, n_chars = 0;
+		for (size_t lo = 0; lo < rows.size(); lo += ROW_BLOCK) {
+			const size_t hi = std::min(rows.size(), lo + (size_t) ROW_BLOCK);
+			pre.assign(hi - lo, row_transcripts()); fill.assign(hi - lo, filled_row());
+			// (A)
+			for_chunks(lo, hi, CHUNK, [&](size_t, size_t a, size_t b) {
+				for (size_t y = a; y < b; ++y) { side_strings sides; transcripts_of_row(rows[y], from_device.get(y, sides) ? &sides : NULL, pre[y - lo]); }
+			});
+			// (B) the distinct transcripts of each side; calls cut at FILL_CHARS characters of bound
+			std::vector<u32> job_row, job_tr; std::vector<u8> job_flags; std::vector<size_t> job_x; // job_x: the row of a job in this block
+			block_chars.clear(); block_pos.clear();
+			size_t x = 0;
+			while (x < hi - lo) {
+				std::string text; std::vector<i32> tpos; std::vector<u32> row_off(1, 0), pos_off(1, 0); u64 bound = 0;
+				job_row.clear(); job_tr.clear(); job_flags.clear(); job_x.clear();
+				for (; x < hi - lo && (bound < (u64) FILL_CHARS || job_row.empty()); ++x) {
+					const row_transcripts& r = pre[x];
+					if (r.t5.empty() && r.t3.empty()) continue;
+					const u32 k = rows[lo + x];
+					bool st5 = e.bits[k] & CB_PSTRAND1, st3 = e.bits[k] & CB_PSTRAND2;
+					if (!(e.bits[k] & CB_TSTART_GENE1)) std::swap(st5, st3);
+					const u8 itd = is_itd(k) ? (u8) ARB_FILL_ITD : (u8) 0;
+					const size_t b5 = r.tseq.find('|'), b3 = r.tseq.rfind('|');
+					const u32 row = (u32) row_off.size() - 1;
+					for (int side = 0; side < 2; ++side) {
+						const std::vector<i32>& ts = side == 0 ? r.t5 : r.t3;
+						for (size_t i = 0; i < ts.size(); ++i) {
+							if (std::find(ts.begin(), ts.begin() + i, ts[i]) != ts.begin() + i) continue; // the best transcript comes twice
+							job_row.push_back(row); job_tr.push_back((u32) ts[i]); job_x.push_back(x);
+							job_flags.push_back((u8) ((side ? ARB_FILL_THREE : 0) | ((side ? st3 : st5) ? ARB_FILL_FORWARD : 0) | itd));
+							bound += fill_bound(ts[i], side ? r.tseq.size() - b3 : b5);
+						}
+					}
+					text += r.tseq; tpos.insert(tpos.end(), r.positions.begin(), r.positions.end()); row_off.push_back((u32) text.size()); pos_off.push_back((u32) tpos.size());
+				}
+				if (job_row.empty()) continue;
+				uint64_t chars = 0;
+				if (arb_fill_gaps(pl.ctx, (u32) row_off.size() - 1, text.data(), row_off.data(), tpos.data(), pos_off.data(), (u32) job_row.size(), job_row.data(), job_tr.data(), job_flags.data(), &chars) != 0) {
+					std::string what = arb_last_error(pl.ctx);
+					const size_t at = what.find("(row "); // name the fusion of the row
+					if (at != std::string::npos) { const u32 r = (u32) atol(what.c_str() + at + 5); for (size_t j = 0; j < job_row.size(); ++j) if (job_row[j] == r) { const u32 k = rows[lo + job_x[j]]; what += " (fusion " + ref.original_names[e.contig1[k]] + ":" + std::to_string((long long) e.bp1[k] + 1) + " / " + ref.original_names[e.contig2[k]] + ":" + std::to_string((long long) e.bp2[k] + 1) + ")"; break; } }
+					throw std::runtime_error("arb_fill_gaps: " + what);
+				}
+				block_chars.emplace_back(chars, '\0'); block_pos.emplace_back(chars + 1);
+				std::vector<u32> off(job_row.size() + 1);
+				if (arb_get_filled(pl.ctx, off.data(), &block_chars.back()[0], block_pos.back().data()) != 0) throw std::runtime_error(std::string("arb_get_filled: ") + arb_last_error(pl.ctx));
+				for (size_t j = 0; j < job_row.size(); ++j) {
+					filled_row& f = fill[job_x[j]];
+					filled_row::half h; h.transcript = (i32) job_tr[j]; h.three = job_flags[j] & ARB_FILL_THREE; h.off = off[j]; h.len = off[j + 1] - off[j];
+					f.halves.push_back(h); f.chars = &block_chars.back(); f.pos = &block_pos.back(); // a row's jobs are all in one call
+				}
+				n_jobs += job_row.size(); n_chars += chars;
+			}
+			laps.lap(which, "gap filling (host A + device B)");
+			// (C)
+			for_chunks(lo, hi, CHUNK, [&](size_t c, size_t a, size_t b) {
+				warning_sink = &out.warnings[c];
+				row_buffer text; text.s.reserve(CHUNK * 4096);
+				for (size_t y = a; y < b; ++y) format_row(text, rows[y], NULL, &pre[y - lo], &fill[y - lo]);
+				out.slices[c].swap(text.s);
+			});
+		}
+		if (getenv("ARB_TRACE")) fprintf(stderr, "[laps] output %-10s gap filling jobs %llu, filled characters %llu\n", which, (unsigned long long) n_jobs, (unsigned long long) n_chars);
 		laps.lap(which, "rows formatted");
 	}
 	static int open_output(const std::string& path) {

@@ -12,7 +12,7 @@ namespace arb { namespace host {
 static double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
 run_options::run_options(): interesting_contigs("1 2 3 4 5 6 7 8 9 10 11 12 13 14 15 16 17 18 19 20 21 22 X Y AC_* NC_*"), viral_contigs("AC_* NC_*"),
-	strandedness(3), fragment_length(200), threads(1), device(0), print_extra_info_for_discarded_fusions(false), min_support(2), min_anchor_length(23), min_spliced_events(4), min_itd_support(10),
+	strandedness(3), fragment_length(200), threads(1), device(0), print_extra_info_for_discarded_fusions(false), fill_sequence_gaps(false), min_support(2), min_anchor_length(23), min_spliced_events(4), min_itd_support(10),
 	high_expression_quantile(0.998f), exonic_fraction(0.33f), min_itd_allele_fraction(0.07f), echo_progress(false), top_viral_contigs(5), viral_contig_min_covered_fraction(0.05f), max_genomic_breakpoint_distance(100000) { arb_default_params(&params); }
 
 void pipeline::say(const std::string& line) {

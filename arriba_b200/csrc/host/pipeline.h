@@ -32,6 +32,7 @@ struct run_options { // options_t (options.hpp:25-69) restricted to what this im
 	int threads;               // host threads for decode/annotation (the reference's -@ only affects BAM decoding)
 	int device;
 	bool print_extra_info_for_discarded_fusions; // -X
+	bool fill_sequence_gaps; // -I
 	int min_support; unsigned min_anchor_length, min_spliced_events, min_itd_support; float high_expression_quantile, exonic_fraction, min_itd_allele_fraction; bool echo_progress;
 	unsigned top_viral_contigs; float viral_contig_min_covered_fraction; // -T 5, -C 0.05
 	std::string genomic_breakpoints_file; unsigned max_genomic_breakpoint_distance; // -d (empty: none), -D 100000
@@ -91,6 +92,7 @@ struct pipeline {
 	bool mismappers_begin(); void mismappers_end(); double t_mismappers_begin;
 	void ensure_coverage_on_device(); void attach_device(); // a part that only works on replicated device state: a context with the run's parameters
 	bool frags_on_device, reference_on_device, coverage_on_device, row_texts_on_device; u32 contigs_on_device;
+	bool fill_transcripts_on_device = false; // -I: the transcript table of the writer (arb_set_fill_transcripts)
 	void say_read_filter_counts();
 };
 

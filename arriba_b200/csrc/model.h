@@ -62,7 +62,7 @@ struct annot_view {
 	const u32* exon_grid; const u32* exon_grid_begin; const u32* gene_grid; const u32* gene_grid_begin; // host-side search accelerators (annot_hd.h region_find); 0 on the device
 	// contig properties
 	u8* contig_flags;        // bit0 interesting, bit1 viral
-	u64* contig_seq_off;     // offset of the contig's sequence in assembly[]; ~0 if the sequence is not loaded
+	u64* contig_seq_off;     // offset of the contig's sequence in assembly[]; 0 if the sequence is not loaded (then contig_len is 0)
 	u32* contig_len;
 	const char* assembly;    // upper-cased reference bases, 1 byte per base
 	const u32* assembly4;    // the same bases as nt16 codes, 8 per word (first base in the top nibble), same base offsets; 0 if a character outside the nt16 alphabet occurs

@@ -70,7 +70,8 @@ class Timings(C.Structure):
                 ("tags_match_ms", C.c_float), ("tags_sort_ms", C.c_float), ("tags_pairs", C.c_uint64), ("protein_domains_ms", C.c_float),
                 ("rec_chunk_copy_ms", C.c_float), ("rec_chunk_kernels_ms", C.c_float), ("rec_sort_ms", C.c_float), ("rec_count_ms", C.c_float),
                 ("rec_scan_ms", C.c_float), ("rec_write_ms", C.c_float), ("rec_download_ms", C.c_float),
-                ("rec_text_parse_ms", C.c_float)]
+                ("rec_text_parse_ms", C.c_float), ("fill_gaps_ms", C.c_float),
+                ("fill_gaps_jobs", C.c_uint64), ("fill_gaps_chars", C.c_uint64)]
 
 
 _CTYPE = {np.dtype(np.uint8): C.c_uint8, np.dtype(np.uint16): C.c_uint16, np.dtype(np.uint32): C.c_uint32, np.dtype(np.int32): C.c_int32,
@@ -143,6 +144,9 @@ def load(path=None):
                        ("arb_set_protein_domains", [C.c_uint32, _p(C.c_uint16), _p(C.c_int32), _p(C.c_int32), _p(C.c_uint32), _p(C.c_uint32), C.c_uint32, C.c_char_p, _p(C.c_uint32)]),
                        ("arb_retained_protein_domains", [C.c_uint32, _p(C.c_uint32), _p(C.c_uint64)]),
                        ("arb_get_retained_protein_domains", [_p(C.c_uint64), C.c_char_p]),
+                       ("arb_set_fill_transcripts", [C.c_uint32, _p(C.c_int32), _p(C.c_int32), _p(C.c_uint32), _p(C.c_int32), _p(C.c_int32)]),
+                       ("arb_fill_gaps", [C.c_uint32, C.c_char_p, _p(C.c_uint32), _p(C.c_int32), _p(C.c_uint32), C.c_uint32, _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint8), _p(C.c_uint64)]),
+                       ("arb_get_filled", [_p(C.c_uint32), C.c_char_p, _p(C.c_int32)]),
                        ("arb_set_candidate_state", [_p(C.c_uint8), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_float)]),
                        ("arb_set_candidate_lists", [_p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32), _p(C.c_uint32)]),
                        ("arb_set_splice_sites", [_p(C.c_uint32), _p(C.c_int32)]),
@@ -435,6 +439,34 @@ class Context:
         raw = text.raw
         return [raw[int(off[x]):int(off[x + 1])] for x in range(ids.size)]
 
+    # ---- gap filling of fusion transcript sequences (-I)
+    FILL_THREE, FILL_FORWARD, FILL_ITD = 1, 2, 4
+
+    def set_fill_transcripts(self, first_exon, last_exon, contig, exon_next, exon_prev):
+        """The transcripts of the resident annotation (first and last exon, contig) and the exon chains (next / previous exon of the same transcript, -1: none)."""
+        t = [np.ascontiguousarray(first_exon, np.int32), np.ascontiguousarray(last_exon, np.int32), np.ascontiguousarray(contig, np.uint32)]
+        e = [np.ascontiguousarray(exon_next, np.int32), np.ascontiguousarray(exon_prev, np.int32)]
+        n = t[0].size
+        assert all(c.size == n for c in t) and e[0].size == e[1].size, "columns differ in length"
+        t = [c if c.size else np.zeros(1, c.dtype) for c in t]; e = [c if c.size else np.zeros(1, c.dtype) for c in e]
+        self._check(self.lib.arb_set_fill_transcripts(self.h, n, *[ptr(c) for c in t], *[ptr(c) for c in e]))
+
+    def fill_gaps(self, sequences, positions, jobs):
+        """Fills the sides of unfilled sequences (bytes, one per row, with the positions of their characters, at least one per character): jobs = (row, transcript, flags) with the
+        FILL_* flags. Returns, per job, the filled side (bytes) and its positions: P5 replaces the sequence before its first '|', S3 the one after its last."""
+        assert len(sequences) == len(positions)
+        row_off = np.zeros(len(sequences) + 1, np.uint32); row_off[1:] = np.cumsum([len(s) for s in sequences]) if sequences else []
+        text = b"".join(sequences) + b"\0"
+        pos = np.concatenate([np.asarray(p, np.int32) for p in positions] + [np.zeros(1, np.int32)])
+        pos_off = np.zeros(len(positions) + 1, np.uint32); pos_off[1:] = np.cumsum([len(p) for p in positions]) if positions else []
+        row = np.array([j[0] for j in jobs] or [0], np.uint32); tr = np.array([j[1] for j in jobs] or [0], np.uint32); fl = np.array([j[2] for j in jobs] or [0], np.uint8)
+        n = C.c_uint64()
+        self._check(self.lib.arb_fill_gaps(self.h, len(sequences), text, ptr(row_off), ptr(pos), ptr(pos_off), len(jobs), ptr(row), ptr(tr), ptr(fl), C.byref(n)))
+        off = np.zeros(len(jobs) + 1, np.uint32); chars = C.create_string_buffer(int(n.value) + 1); out_pos = np.zeros(int(n.value) + 1, np.int32)
+        self._check(self.lib.arb_get_filled(self.h, ptr(off), chars, ptr(out_pos)))
+        raw = chars.raw
+        return [(raw[int(off[j]):int(off[j + 1])], out_pos[int(off[j]):int(off[j + 1])].tolist()) for j in range(len(jobs))]
+
     def slot_swaps(self):
         s = np.zeros(self.n_fragments, np.uint8)
         self._check(self.lib.arb_get_slot_swaps(self.h, ptr(s)))
@@ -498,7 +530,8 @@ class RunOptions(C.Structure):
                 ("print_extra_info_for_discarded_fusions", C.c_int32), ("echo_progress", C.c_int32),
                 ("top_viral_contigs", C.c_uint32), ("viral_contig_min_covered_fraction", C.c_float),
                 ("genomic_breakpoints_file", C.c_char_p), ("max_genomic_breakpoint_distance", C.c_uint32), ("blacklist_file", C.c_char_p),
-                ("known_fusions_file", C.c_char_p), ("tags_file", C.c_char_p), ("protein_domains_file", C.c_char_p), ("chimeric_file", C.c_char_p)]
+                ("known_fusions_file", C.c_char_p), ("tags_file", C.c_char_p), ("protein_domains_file", C.c_char_p), ("chimeric_file", C.c_char_p),
+                ("fill_sequence_gaps", C.c_int32)]
 
 
 class RunStats(C.Structure):
@@ -549,7 +582,7 @@ class Pipeline:
 
     def __init__(self, bam, gtf, fasta, threads=1, device=0, lib_path=None, strandedness=3, params=None, output=None, discarded=None,
                  genomic_breakpoints=None, max_genomic_breakpoint_distance=100000, blacklist=None, known_fusions=None, tags=None, protein_domains=None,
-                 chimeric=None):
+                 chimeric=None, fill_sequence_gaps=False, extra_info=False, interesting_contigs=None):
         self.lib = load(lib_path)
         _load_pipeline_api(self.lib)
         o = RunOptions()
@@ -573,6 +606,10 @@ class Pipeline:
             self._strings.append(protein_domains.encode()); o.protein_domains_file = self._strings[-1]
         if chimeric:
             self._strings.append(chimeric.encode()); o.chimeric_file = self._strings[-1]
+        o.fill_sequence_gaps = int(bool(fill_sequence_gaps))  # -I
+        o.print_extra_info_for_discarded_fusions = int(bool(extra_info))  # -X
+        if interesting_contigs is not None:  # -i: a list of contig names
+            self._strings.append(" ".join(interesting_contigs).encode()); o.interesting_contigs = self._strings[-1]
         o.threads = threads; o.device = device; o.strandedness = strandedness
         if params is not None:
             o.params = params

@@ -409,6 +409,22 @@ int arb_set_protein_domains(arb_ctx* ctx, uint32_t n, const uint16_t* contig, co
 int arb_retained_protein_domains(arb_ctx* ctx, uint32_t n_ids, const uint32_t* ids, uint64_t* n_bytes);
 int arb_get_retained_protein_domains(arb_ctx* ctx, uint64_t* off, char* text);
 
+/* ---- gap filling of fusion transcript sequences (-I) ------------------------------------------------------------------------------------------------------
+ * These replace fill_gaps_in_fusion_transcript_sequence (source/output_fusions.cpp:820-1041). Its 5' part rewrites only the characters before the first '|' of
+ * the sequence, its 3' part only those after the last '|', so each side is a job of its own: (row, transcript, flags), flags = ARB_FILL_THREE for the 3' side
+ * (else 5'), ARB_FILL_FORWARD when the side's predicted strand is forward, ARB_FILL_ITD when the row is an internal tandem duplication. The filled sequence
+ * of a transcript pair is then P5 + seq[b5 .. b3] + S3 (b5: first '|', b3: last '|'), P5 the output of the pair's 5' job, S3 that of its 3' job.
+ * arb_set_fill_transcripts: the n transcripts of the resident annotation (first and last exon, contig) and the exon chains (next / previous exon of the same
+ * transcript, -1: none; one entry per exon of the annotation). arb_fill_gaps: the rows' unfilled sequences text[row_off[r] .. row_off[r + 1]) and the positions
+ * of their characters pos[pos_off[r] .. pos_off[r + 1]) (-1: none; at least one per character, and more where the writer keeps more, indexed like the
+ * text); *n_chars is the size of all outputs. arb_get_filled returns them: off[n_jobs + 1], the characters and their
+ * positions, job j at [off[j] .. off[j + 1]). A transcript whose exons reach beyond its contig's sequence stops arb_fill_gaps with an error naming the job. */
+enum { ARB_FILL_THREE = 1, ARB_FILL_FORWARD = 2, ARB_FILL_ITD = 4 };
+int arb_set_fill_transcripts(arb_ctx* ctx, uint32_t n, const int32_t* first_exon, const int32_t* last_exon, const uint32_t* contig, const int32_t* exon_next, const int32_t* exon_prev);
+int arb_fill_gaps(arb_ctx* ctx, uint32_t n_rows, const char* text, const uint32_t* row_off, const int32_t* pos, const uint32_t* pos_off, uint32_t n_jobs, const uint32_t* row, const uint32_t* transcript,
+                  const uint8_t* flags, uint64_t* n_chars);
+int arb_get_filled(arb_ctx* ctx, uint32_t* off, char* chars, int32_t* pos);
+
 /* ---- device timing (CUDA events recorded on the context's stream around each stage) ---------------------------------- */
 typedef struct arb_timings {
 	float duplicates_ms;        /* duplicate marking (key build + hash group-by + mark) */
@@ -455,6 +471,8 @@ typedef struct arb_timings {
 	float rec_write_ms;         /* the writing replay launches (pools and coverage counts) */
 	float rec_download_ms;      /* the coverage windows packed and brought back with the counters */
 	float rec_text_parse_ms;    /* SAM input, part of rec_chunk_kernels_ms: line ends, the parse and the staged BAM records, summed over the chunks */
+	float fill_gaps_ms;         /* -I: arb_set_fill_transcripts plus every arb_fill_gaps since (copies of the jobs, plan, scan and the filled sequences) */
+	uint64_t fill_gaps_jobs, fill_gaps_chars; /* -I: the jobs of every arb_fill_gaps and the characters they wrote */
 } arb_timings;
 int arb_get_timings(arb_ctx* ctx, arb_timings* out);
 /* Device scratch memory is pooled per device and survives arb_ctx_destroy so that the next sample reuses it; this returns it to the driver
@@ -500,6 +518,7 @@ typedef struct arb_run_options {
 	const char* tags_file;           /* -t: tags (optionally .gz), NULL = none */
 	const char* protein_domains_file; /* -p: protein domains (GFF3, optionally .gz), NULL = none */
 	const char* chimeric_file;       /* -c: STAR's Chimeric.out.sam (SAM, BGZF SAM or BAM; --chimOutType SeparateSAMold), NULL = none */
+	int32_t fill_sequence_gaps;      /* -I */
 } arb_run_options;
 void arb_default_run_options(arb_run_options* o);
 

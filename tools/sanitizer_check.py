@@ -3,6 +3,7 @@
 as the kernels, every device buffer its own malloc) and of the `arriba` front end with -fsanitize=address,undefined and runs worlds through it. An index that
 runs past a column is silent on the GPU; here it stops the run. Test infrastructure; nothing of it is linked into the product.
     python tools/sanitizer_check.py OUTDIR PREFIX [ENV=VALUE ...] [PREFIX ...]      # PREFIX.bam / .gtf / .fa; ENV=VALUE pairs apply to the prefix before them
+    python tools/sanitizer_check.py OUTDIR PREFIX "ARGS=-I -X" ...                 # ARGS=...: more command-line options for that run (here: gap filling)
     SANITIZE=thread python tools/sanitizer_check.py ...                                # ThreadSanitizer instead: races between the host threads (THREADS=n for -@)"""
 import os, subprocess, sys
 from concurrent.futures import ThreadPoolExecutor
@@ -40,11 +41,12 @@ def main():
             runs.append((a, {}))
     bad = 0
     for i, (prefix, extra) in enumerate(runs):
+        extra = dict(extra); args = extra.pop("ARGS", "").split()
         env = dict(os.environ, ASAN_OPTIONS="detect_leaks=0:halt_on_error=1", UBSAN_OPTIONS="print_stacktrace=1:halt_on_error=1", TSAN_OPTIONS="halt_on_error=0 report_signal_unsafe=0", **extra)
-        r = subprocess.run([exe, "-x", prefix + ".bam", "-g", prefix + ".gtf", "-a", prefix + ".fa", "-o", os.path.join(out, "%d.tsv" % i), "-O", os.path.join(out, "%d.discarded.tsv" % i), "-f", "blacklist", "-@", os.environ.get("THREADS", "5")],
+        r = subprocess.run([exe, "-x", prefix + ".bam", "-g", prefix + ".gtf", "-a", prefix + ".fa", "-o", os.path.join(out, "%d.tsv" % i), "-O", os.path.join(out, "%d.discarded.tsv" % i), "-f", "blacklist", "-@", os.environ.get("THREADS", "5")] + args,
                            env=env, stdout=subprocess.DEVNULL, stderr=subprocess.PIPE, text=True)
         reports = [l for l in r.stderr.splitlines() if "AddressSanitizer" in l or "runtime error" in l or "WARNING: ThreadSanitizer" in l]
-        print("%s %s: exit code %d, sanitizer reports %d" % (prefix, extra, r.returncode, len(reports)), flush=True)
+        print("%s %s %s: exit code %d, sanitizer reports %d" % (prefix, " ".join(args), extra, r.returncode, len(reports)), flush=True)
         for l in reports[:5]:
             print("   ", l)
         bad += bool(reports) or r.returncode != 0
