@@ -113,6 +113,9 @@ int arb_records_begin(arb_ctx* ctx, const uint16_t* tid_to_contig, uint32_t n_ti
 int arb_records_chunk(arb_ctx* ctx, const uint8_t* chunk, uint64_t bytes, uint64_t first, uint64_t chunk_pos, uint64_t* n_records, uint64_t* carry, uint32_t* malformed, uint64_t* error) {
 	ARB_API_BEGIN(ctx) u64 r = 0, c = 0, e = 0; ctx->e.records_chunk(chunk, bytes, first, chunk_pos, &r, &c, malformed, &e); *n_records = r; *carry = c; *error = e; ARB_API_END(ctx)
 }
+int arb_records_bgzf_stage(arb_ctx* ctx, const uint8_t* raw, uint64_t raw_bytes, const arb_bgzf_block* blocks, uint32_t n_blocks) {
+	ARB_API_BEGIN(ctx) if (n_blocks && !blocks) throw arb_error("arb_records_bgzf_stage: no block table"); ctx->e.records_bgzf_stage(raw, raw_bytes, blocks, n_blocks); ARB_API_END(ctx)
+}
 int arb_records_source(arb_ctx* ctx, int chimeric_file, const uint16_t* tid_to_contig, uint32_t n_tid, uint64_t* first_position) {
 	ARB_API_BEGIN(ctx) u64 f = 0; ctx->e.records_source(chimeric_file != 0, tid_to_contig, n_tid, &f); *first_position = f; ARB_API_END(ctx)
 }
@@ -190,6 +193,7 @@ int arb_filter_mismappers_part(arb_ctx* ctx, int32_t max_mate_gap, int part, int
 int arb_filter_mismappers_finish(arb_ctx* ctx, uint64_t* n) { ARB_API_BEGIN(ctx) const uint64_t k = ctx->e.filter_mismappers_finish(); if (n) *n = k; ARB_API_END(ctx) }
 int arb_get_timings(arb_ctx* ctx, arb_timings* out) { ARB_API_BEGIN(ctx) *out = ctx->e.timings; ARB_API_END(ctx) }
 int arb_selftest_mismatch_counts(arb_ctx* ctx, uint32_t* out) { ARB_API_BEGIN(ctx) ctx->e.probe_mismatch_counts(out); ARB_API_END(ctx) } // tests only, not declared in the public header
+int arb_selftest_staged_chunk(arb_ctx* ctx, uint8_t* out, uint64_t n) { ARB_API_BEGIN(ctx) if (!ctx->e.rec_stage_pending || n > ctx->e.rec_carry + ctx->e.rec_staged) throw arb_error("no staged chunk of that size"); ctx->e.bam_buf.download(ctx->e.ex, out, n); ARB_API_END(ctx) } // tests only, as above: the chunk arb_records_bgzf_stage assembled, behind the carried record
 int arb_selftest_kmer_lookup(arb_ctx* ctx, const uint32_t* contig, const uint32_t* kmer, const int32_t* from, uint32_t n, uint32_t* out) { ARB_API_BEGIN(ctx) ctx->e.probe_kmer_lookup(contig, kmer, from, n, out); ARB_API_END(ctx) } // tests only, as above
 int arb_set_genomic_breakpoints(arb_ctx* ctx, uint32_t n, const uint16_t* c1, const uint16_t* c2, const uint8_t* d1, const uint8_t* d2, const int32_t* p1, const int32_t* p2) {
 	ARB_API_BEGIN(ctx) ctx->e.set_genomic_breakpoints(n, c1, c2, d1, d2, p1, p2); ARB_API_END(ctx)

@@ -152,6 +152,10 @@ public:
 	void records_chunk(const u8* chunk, u64 bytes, u64 first, u64 chunk_pos, u64* n_records, u64* carry, u32* malformed, u64* error);
 	void records_finish(u16* const* coverage, u8* const* starts, u8* const* ends, u64* counters, u64* error);
 	u64 records_upload(const u8* chunk, u64 bytes);
+	// stream input: the inflated chunk assembled on the device from the raw BGZF blocks (stage_hd.h); the next records_chunk / records_text_chunk with
+	// chunk == NULL takes it
+	void records_bgzf_stage(const u8* raw, u64 raw_bytes, const arb_bgzf_block* blocks, u32 n_blocks);
+	dbuf<u8> rec_raw; dbuf<arb_bgzf_block> rec_stage_blocks; u64 rec_staged = 0; bool rec_stage_pending = false;
 	void records_store(const dbuf<u8>& B, u64 buf_pos, u64 total, const u32* rec_off, u32 R, u64 seen, u64* error);
 	// SAM text input (samscan.cu): lines staged as BAM records, then records_store
 	void records_text_names(const char* names, const u64* name_off, u32 n);

@@ -36,8 +36,9 @@ static const char* FILTERS[] = {"", "duplicates", "inconsistently_clipped", "hom
 static void usage() {
 	std::cout << "arriba-b200: H100-native implementation of Arriba's post-alignment path (reference version 2.5.1 semantics)\n\n"
 	          << "Usage: arriba [-c Chimeric.out.sam] -x Aligned.out.bam -g annotation.gtf -a assembly.fa -o fusions.tsv [-O fusions.discarded.tsv] [OPTIONS]\n\n"
-	          << " -x FILE  BAM or SAM (plain or BGZF) with main and chimeric alignments (STAR --chimOutType WithinBAM)\n"
-	          << " -c FILE  chimeric alignments in a separate file (STAR --chimOutType SeparateSAMold: Chimeric.out.sam; SAM, BGZF SAM or BAM), read before -x\n"
+	          << " -x FILE  BAM or SAM (plain or BGZF) with main and chimeric alignments (STAR --chimOutType WithinBAM); a pipe is read as it arrives:\n"
+	          << "          STAR ... --outStd BAM_Unsorted --outBAMcompression 0 | arriba -x /dev/stdin ...\n"
+	          << " -c FILE  chimeric alignments in a separate file (STAR --chimOutType SeparateSAMold: Chimeric.out.sam; SAM, BGZF SAM or BAM; a file or a pipe), read before -x\n"
 	          << " -g FILE  gene annotation (GTF)\n -a FILE  assembly (FastA)\n"
 	          << " -o FILE  output file   -O FILE  discarded candidates\n -f LIST  disable filters (comma/space separated)\n -s MODE  strandedness auto|yes|no|reverse\n"
 	          << " -i/-v contig lists, -E e-value cutoff, -S min support, -m/-L/-H/-R/-A/-M/-K/-V/-F/-U/-Q/-e/-l/-z/-Z thresholds as in the reference\n"

@@ -1,11 +1,13 @@
 // ingest.cpp -- see ingest.h. BGZF blocks (or pieces of a plain SAM file) are copied into chunks in parallel on the host and the header (BAM, or SAM's @ lines) is read here; everything the reference's record loop does
-// runs on the device (csrc/records.cu), and so does the fragment table (csrc/fragtable.cu).
+// runs on the device (csrc/records.cu), and so does the fragment table (csrc/fragtable.cu). An input that is not a regular file (a pipe: STAR ... | arriba
+// -x /dev/stdin) is read in sequence into the chunks; its BGZF blocks go to the device as they were read, and the device assembles the inflated chunk.
 #include "ingest.h"
 #include "../../../include/arriba_b200.h"
 #include <set>
 #include "../records_hd.h"
 #include <zlib.h>
 #include <fcntl.h>
+#include <errno.h>
 #include <sys/mman.h>
 #include <sys/stat.h>
 #include <unistd.h>
@@ -108,6 +110,22 @@ int coverage_windows::get_coverage(u32 contig, i32 position, u32 direction) cons
 }
 
 // ------------------------------------------------------------------------------------------- BGZF container
+// STAR is run with --outBAMcompression 0 (run_arriba.sh:34): every BGZF block then holds ONE stored deflate block -- header byte 0x01 (final, type 00),
+// LEN, ~LEN, the bytes (RFC 1951 3.2.4). Is the payload `in` (in_len bytes, out_len inflated) such a block?
+static bool stored_block(const u8* in, u32 in_len, u32 out_len) {
+	return in_len == 5ull + out_len && in[0] == 0x01 && rd16(in + 1) == (u16) out_len && (u16) (rd16(in + 1) ^ rd16(in + 3)) == 0xFFFF;
+}
+static void inflate_payload(const u8* in, u32 in_len, u32 out_len, u8* dst) {
+	if (out_len == 0) return;
+	if (stored_block(in, in_len, out_len)) { memcpy(dst, in + 5, out_len); return; } // copied; anything else goes through zlib
+	z_stream zs; memset(&zs, 0, sizeof(zs));
+	if (inflateInit2(&zs, -15) != Z_OK) fail("failed to load alignments");
+	zs.next_in = (Bytef*) in; zs.avail_in = in_len; zs.next_out = dst; zs.avail_out = out_len;
+	const int rc = inflate(&zs, Z_FINISH);
+	inflateEnd(&zs);
+	if (rc != Z_STREAM_END || zs.avail_out != 0) fail("failed to load alignments");
+}
+
 struct bgzf_file {
 	const u8* data; size_t size; int fd;
 	struct block { u64 in_off; u32 in_len; u32 out_len; u64 out_off; };
@@ -115,15 +133,19 @@ struct bgzf_file {
 	bgzf_file(): data(NULL), size(0), fd(-1), total_out(0), raw(false) {}
 	~bgzf_file() { if (data) munmap((void*) data, size); if (fd >= 0) close(fd); }
 	bool raw; // plain SAM text: the "blocks" are pieces of the file, copied as they are
-	void map(const std::string& path) {
+	// A regular file is mapped (true). Anything else that can be read in sequence (a pipe, a FIFO, a character device) is left open in fd for the
+	// stream reader (false).
+	bool map(const std::string& path) {
 		fd = ::open(path.c_str(), O_RDONLY);
 		if (fd < 0) fail("failed to open SAM file");
-		struct stat st; fstat(fd, &st); size = st.st_size;
-		if (!S_ISREG(st.st_mode)) fail("failed to open SAM file (input from a pipe or device is not supported: pass a regular file)");
+		struct stat st; if (fstat(fd, &st) != 0 || S_ISDIR(st.st_mode)) fail("failed to open SAM file");
+		size = st.st_size;
+		if (!S_ISREG(st.st_mode)) { size = 0; return false; }
 		if (size == 0) fail("failed to read SAM header");
 		data = (const u8*) mmap(NULL, size, PROT_READ, MAP_PRIVATE, fd, 0);
 		if (data == MAP_FAILED) { data = NULL; fail("failed to open SAM file"); }
 		madvise((void*) data, size, MADV_SEQUENTIAL);
+		return true;
 	}
 	void raw_pieces(u64 piece) {
 		raw = true;
@@ -191,16 +213,7 @@ struct bgzf_file {
 	void inflate_block(const block& b, u8* dst) const {
 		if (b.out_len == 0) return;
 		if (raw) { memcpy(dst, data + b.in_off, b.out_len); return; }
-		// STAR is run with --outBAMcompression 0 (run_arriba.sh:34): every BGZF block then holds ONE stored deflate block -- header byte 0x01 (final, type 00),
-		// LEN, ~LEN, the bytes (RFC 1951 3.2.4). Those are copied; anything else goes through zlib.
-		const u8* const in = data + b.in_off;
-		if (b.in_len == 5ull + b.out_len && in[0] == 0x01 && rd16(in + 1) == (u16) b.out_len && (u16) (rd16(in + 1) ^ rd16(in + 3)) == 0xFFFF) { memcpy(dst, in + 5, b.out_len); return; }
-		z_stream zs; memset(&zs, 0, sizeof(zs));
-		if (inflateInit2(&zs, -15) != Z_OK) fail("failed to load alignments");
-		zs.next_in = (Bytef*) (data + b.in_off); zs.avail_in = b.in_len; zs.next_out = dst; zs.avail_out = b.out_len;
-		const int rc = inflate(&zs, Z_FINISH);
-		inflateEnd(&zs);
-		if (rc != Z_STREAM_END || zs.avail_out != 0) fail("failed to load alignments");
+		inflate_payload(data + b.in_off, b.in_len, b.out_len, dst);
 	}
 };
 
@@ -246,40 +259,152 @@ static std::string record_error_text(u64 error, arb_ctx* ctx, const std::vector<
 	return "failed to load alignments";
 }
 
-// The format is decided by the file's content, as htslib's sam_open does: BGZF whose stream starts with "BAM\1" is BAM, any other BGZF stream is SAM
-// text, and a file that is not gzip is plain SAM if its first line starts with '@' or has at least 10 tabs. The block table is built here (BGZF), or the
-// file is cut into pieces of at most 4 MiB, and no larger than a chunk (but at least 256 bytes), that are copied as they are (plain SAM).
+// The format is decided by the input's content, as htslib's sam_open does: BGZF whose stream starts with "BAM\1" is BAM, any other BGZF stream is SAM
+// text, and an input that is not gzip is plain SAM if its first line starts with '@' or has at least 10 tabs. detect_prefix_bgzf is that rule over the first
+// bytes: all of a shorter input, for a gzip input its first header, else at least its first line. Files and streams both call it.
 enum input_format { INPUT_BAM, INPUT_SAM_BGZF, INPUT_SAM };
-static input_format detect_format(bgzf_file& f, int threads, u64 chunk_target) {
-	const u8* d = f.data;
-	if (f.size >= 3 && d[0] == 0x1f && d[1] == 0x8b && d[2] == 8) {
-		const u32 xlen = f.size >= 12 ? rd16(d + 10) : 0;
+static bool detect_prefix_bgzf(const u8* d, size_t n) { // true: BGZF (BAM or SAM); false: plain SAM
+	if (n >= 3 && d[0] == 0x1f && d[1] == 0x8b && d[2] == 8) {
+		const u32 xlen = n >= 12 ? rd16(d + 10) : 0;
 		bool bgzf = false;
-		if ((d[3] & 4) && f.size >= 12ull + xlen)
+		if (n >= 4 && (d[3] & 4) && n >= 12ull + xlen)
 			for (u32 x = 0; x + 4 <= xlen;) { const u8* e = d + 12 + x; if (e[0] == 'B' && e[1] == 'C') bgzf = true; x += 4 + rd16(e + 2); }
 		if (!bgzf) fail("failed to read SAM header (gzip-compressed SAM must be BGZF (bgzip) or uncompressed)");
-		f.block_table(threads);
-		std::vector<u8> head;
-		for (size_t b = 0; b < f.blocks.size() && head.size() < 4; ++b) { const size_t at = head.size(); head.resize(at + f.blocks[b].out_len); f.inflate_block(f.blocks[b], head.data() + at); }
-		return head.size() >= 4 && memcmp(head.data(), "BAM\1", 4) == 0 ? INPUT_BAM : INPUT_SAM_BGZF;
+		return true;
 	}
-	if (f.size >= 4 && memcmp(d, "CRAM", 4) == 0) fail("failed to read SAM header (CRAM input is not supported: convert it to BAM or SAM)");
+	if (n >= 4 && memcmp(d, "CRAM", 4) == 0) fail("failed to read SAM header (CRAM input is not supported: convert it to BAM or SAM)");
 	u32 tabs = 0;
-	for (size_t x = 0; x < f.size && d[x] != '\n'; ++x) tabs += d[x] == '\t';
-	if (d[0] != '@' && tabs < 10) fail("failed to read SAM header");
-	f.raw_pieces(std::max<u64>(256, std::min<u64>(chunk_target, 4ull << 20)));
-	return INPUT_SAM;
+	for (size_t x = 0; x < n && d[x] != '\n'; ++x) tabs += d[x] == '\t';
+	if (n == 0 || (d[0] != '@' && tabs < 10)) fail("failed to read SAM header");
+	return false;
+}
+// BAM or SAM, from the first inflated bytes of a BGZF input
+template <class S> static input_format bgzf_format(S& src) {
+	std::vector<u8> head;
+	while (head.size() < 4 && src.more(head)) {}
+	src.rewind();
+	return head.size() >= 4 && memcmp(head.data(), "BAM\1", 4) == 0 ? INPUT_BAM : INPUT_SAM_BGZF;
 }
 
-// The @ lines at the start of a SAM stream, however many blocks they span; every @SQ line gives the next reference (its SN) to `reference`. Returns the
-// offset of the first record in the stream.
-template <class F> static u64 read_sam_header(const bgzf_file& f, F reference) {
-	std::string text; size_t inflated = 0;
-	auto more = [&]() {
-		if (inflated >= f.blocks.size()) return false;
-		const size_t at = text.size(); text.resize(at + f.blocks[inflated].out_len); f.inflate_block(f.blocks[inflated], (u8*) &text[at]); ++inflated;
+// The inflated bytes of an input from its start, one block (or piece of plain text) at a time, for format detection and the header: more() appends the
+// next one (false at the end), available(n): the input holds at least n inflated bytes, rewind(): more() starts again at the first block.
+struct file_source {
+	const bgzf_file& f; size_t next;
+	explicit file_source(const bgzf_file& file): f(file), next(0) {}
+	template <class B> bool more(B& out) {
+		if (next >= f.blocks.size()) return false;
+		const size_t at = out.size(); out.resize(at + f.blocks[next].out_len); f.inflate_block(f.blocks[next], (u8*) &out[at]); ++next;
 		return true;
-	};
+	}
+	bool available(u64 n) const { return n <= f.total_out; }
+	void rewind() { next = 0; }
+};
+
+// A block header as the file path's block table judges it, at d[0, n) of an input read in sequence (at_eof: no more bytes will come): 1 = a whole block
+// (bsize, xlen), 0 = more bytes are needed to tell, -1 = the end of the blocks (fewer than 18 bytes left: the block table ignores them). A malformed
+// header stops the run with a framing_error, which no other error of the input outranks (the file path checks the framing of the whole file first).
+struct framing_error: std::runtime_error { explicit framing_error(const std::string& m): std::runtime_error(m) {} };
+static int stream_block_at(const u8* d, size_t n, bool at_eof, u32& bsize, u32& xlen) {
+	if (n < 18) return at_eof ? -1 : 0;
+	if (!(d[0] == 0x1f && d[1] == 0x8b && d[2] == 8 && (d[3] & 4))) throw framing_error("failed to load alignments");
+	xlen = rd16(d + 10);
+	if (n < 12ull + xlen + 2 && !at_eof) return 0;
+	bool found = false;
+	for (u32 x = 0; x + 4 <= xlen && 12ull + x + 6 <= n;) { const u8* e = d + 12 + x; const u32 slen = rd16(e + 2); if (e[0] == 'B' && e[1] == 'C' && slen == 2) { bsize = rd16(e + 4) + 1u; found = true; } x += 4 + slen; }
+	if (!found || bsize < 12 + xlen + 8) throw framing_error("failed to load alignments");
+	if (bsize > n) { if (!at_eof) return 0; throw framing_error("failed to load alignments"); }
+	return 1;
+}
+
+// ------------------------------------------------------------------------------------------- stream input
+// An input that is not a regular file: read in sequence. Format detection and the header read into `head`, and what they read beyond the header stays
+// there for the first chunk; the chunks are read into the page-locked chunk buffers. `left` / `n_left`: the bytes read but not yet put into a chunk (in
+// `head`, or behind the blocks of the last chunk in its buffer).
+struct stream_input {
+	int fd; bool eof, started, bgzf;
+	std::vector<u8> head; size_t head_walk; // BGZF: head[head_walk, ...) is not walked yet (header phase)
+	bool in_head;
+	const u8* left; size_t n_left;
+	u64 out_pos; // inflated (plain: stream) position of the first byte behind the last chunk
+	struct block { size_t start; u32 in_off, in_len, out_len; u64 out_off; };
+	std::vector<block> walked; u64 walked_out; size_t inflated; // the header phase's blocks
+	stream_input(int f): fd(f), eof(false), started(false), bgzf(false), head_walk(0), in_head(true), left(NULL), n_left(0), out_pos(0), walked_out(0), inflated(0) {}
+	~stream_input() { if (fd >= 0) close(fd); } // a producer still writing gets EPIPE
+	size_t read_some(u8* dst, size_t n) { // 0: end of the input
+		for (;;) {
+			const ssize_t r = ::read(fd, dst, n);
+			if (r > 0) { started = true; return (size_t) r; }
+			if (r == 0) { eof = true; return 0; }
+			if (errno == EINTR) continue;
+			fail(started ? "failed to load alignments" : "failed to open SAM file");
+		}
+	}
+	bool read_head() { const size_t at = head.size(); head.resize(at + (64u << 10)); const size_t got = eof ? 0 : read_some(head.data() + at, 64u << 10); head.resize(at + got); return got > 0; }
+	// format detection: the bytes detect_prefix_bgzf looks at
+	bool detect() {
+		auto fill = [&](size_t n) { while (head.size() < n && read_head()) {} };
+		fill(4);
+		if (head.size() >= 3 && head[0] == 0x1f && head[1] == 0x8b && head[2] == 8) { fill(12); if (head.size() >= 12) fill(12 + (size_t) rd16(head.data() + 10)); }
+		else for (size_t scanned = 0; !memchr(head.data() + scanned, '\n', head.size() - scanned);) { scanned = head.size(); if (!read_head()) break; }
+		bgzf = detect_prefix_bgzf(head.data(), head.size());
+		return bgzf;
+	}
+	// header phase, BGZF: walk the next block of head (reading as needed); false at the end of the blocks
+	bool walk_one() {
+		u32 bsize = 0, xlen = 0; int r;
+		while ((r = stream_block_at(head.data() + head_walk, head.size() - head_walk, eof, bsize, xlen)) == 0) read_head();
+		if (r < 0) return false;
+		block b; b.start = head_walk; b.in_off = (u32) (12 + xlen); b.in_len = bsize - 20 - xlen; b.out_len = rd32(head.data() + head_walk + bsize - 4); b.out_off = walked_out;
+		walked.push_back(b); walked_out += b.out_len; head_walk += bsize;
+		return true;
+	}
+	// the source of format detection and the header (file_source's interface)
+	template <class B> bool more(B& out) {
+		if (!bgzf) { // plain text: whatever is read next
+			if (head_walk >= head.size() && !read_head()) return false;
+			const size_t at = out.size(); out.resize(at + head.size() - head_walk); memcpy(&out[at], head.data() + head_walk, head.size() - head_walk); head_walk = head.size();
+			return true;
+		}
+		if (inflated >= walked.size() && !walk_one()) return false;
+		const block& b = walked[inflated++];
+		const size_t at = out.size(); out.resize(at + b.out_len); inflate_payload(head.data() + b.start + b.in_off, b.in_len, b.out_len, (u8*) &out[at]);
+		return true;
+	}
+	bool available(u64 n) { while (walked_out < n && walk_one()) {} return walked_out >= n; }
+	void rewind() { inflated = 0; if (!bgzf) head_walk = 0; }
+	// the header ends at header_end: the first chunk starts at the block of the first record (plain text: at the piece of the file path that holds it)
+	void header_done(u64 header_end, u64 piece) {
+		size_t start = head_walk; out_pos = walked_out;
+		if (bgzf) { for (size_t k = 0; k < walked.size(); ++k) if (walked[k].out_off + walked[k].out_len > header_end) { start = walked[k].start; out_pos = walked[k].out_off; break; } }
+		else { out_pos = header_end / piece * piece; start = (size_t) out_pos; }
+		in_head = false; left = head.data() + start; n_left = head.size() - start;
+	}
+	// where the records stop (after an error, or at the end): the framing of the rest of the input is checked (not inflated), as the file path checks it
+	// before anything else. Called while `left` still points into a live chunk buffer; afterwards nothing of the input is read any more.
+	bool drained = false;
+	void drain() {
+		if (!bgzf || drained) return;
+		drained = true;
+		std::vector<u8> w;
+		if (in_head) w.assign(head.begin() + head_walk, head.end()); else w.assign(left, left + n_left);
+		in_head = false; left = NULL; n_left = 0;
+		size_t at = 0;
+		for (;;) {
+			u32 bsize = 0, xlen = 0;
+			const int r = stream_block_at(w.data() + at, w.size() - at, eof, bsize, xlen);
+			if (r < 0) return;
+			if (r > 0) { at += bsize; continue; }
+			w.erase(w.begin(), w.begin() + at); at = 0;
+			const size_t have = w.size(); w.resize(have + (256u << 10)); w.resize(have + read_some(w.data() + have, 256u << 10));
+		}
+	}
+};
+
+// The @ lines at the start of a SAM stream, however many blocks they span; every @SQ line gives the next reference (its SN) to `reference`. Returns the
+// offset of the first record in the stream. src: file_source or stream_input.
+template <class S, class F> static u64 read_sam_header(S& src, F reference) {
+	std::string text;
+	auto more = [&]() { return src.more(text); };
 	size_t p = 0;
 	for (;;) {
 		while (p >= text.size() && more()) {}
@@ -311,11 +436,11 @@ template <class F> static u64 read_sam_header(const bgzf_file& f, F reference) {
 
 // The BAM header (magic, text, references), however many blocks it spans; every reference's name goes to `reference`. Returns the offset of the first
 // record in the inflated stream.
-template <class F> static u64 read_bam_header(const bgzf_file& f, F reference) {
-	std::vector<u8> h; size_t inflated = 0;
+template <class S, class F> static u64 read_bam_header(S& src, F reference) {
+	std::vector<u8> h;
 	auto have = [&](u64 n) { // the first n bytes of the stream are in h
-		if (n > f.total_out) return false;
-		while (h.size() < n && inflated < f.blocks.size()) { const size_t at = h.size(); h.resize(at + f.blocks[inflated].out_len); f.inflate_block(f.blocks[inflated], h.data() + at); ++inflated; }
+		if (!src.available(n)) return false;
+		while (h.size() < n && src.more(h)) {}
 		return h.size() >= n;
 	};
 	if (!have(12) || memcmp(h.data(), "BAM\1", 4) != 0) fail("failed to read SAM header");
@@ -331,24 +456,59 @@ template <class F> static u64 read_bam_header(const bgzf_file& f, F reference) {
 	return p;
 }
 
-// one input file: its blocks, format and header (the contig id of every reference; SAM: the @SQ names, for the RNAME lookup on the device)
+// one input: its blocks (a file) or its reader (a stream), format and header (the contig id of every reference; SAM: the @SQ names, for the RNAME lookup
+// on the device)
 struct input_file {
-	bgzf_file f; input_format format; u64 header_end; std::vector<u16> tid_to_contig; std::string sq_names; std::vector<u64> sq_off;
+	bgzf_file f; std::unique_ptr<stream_input> stream; input_format format; u64 header_end; std::vector<u16> tid_to_contig; std::string sq_names; std::vector<u64> sq_off;
 	input_file(): format(INPUT_BAM), header_end(0), sq_off(1, 0) {}
+	// opened and its format detected: a file's block table is built here (the framing of the whole file is checked), or it is cut into pieces of at most
+	// 4 MiB, and no larger than a chunk (but at least 256 bytes), that are copied as they are (plain SAM); a stream is read as far as the rule needs
+	void open(const std::string& path, int threads, u64 chunk_target) {
+		if (!f.map(path)) {
+			stream.reset(new stream_input(f.fd)); f.fd = -1;
+			if (!stream->detect()) { format = INPUT_SAM; return; }
+			try { format = bgzf_format(*stream); } catch (const framing_error&) { throw; } catch (const std::exception&) { stream->drain(); throw; }
+			return;
+		}
+		if (!detect_prefix_bgzf(f.data, f.size)) { f.raw_pieces(piece(chunk_target)); format = INPUT_SAM; return; }
+		f.block_table(threads);
+		file_source src(f);
+		format = bgzf_format(src);
+	}
+	static u64 piece(u64 chunk_target) { return std::max<u64>(256, std::min<u64>(chunk_target, 4ull << 20)); }
+	bool has_blocks() const { return stream ? !stream->bgzf || !stream->walked.empty() : !f.blocks.empty(); }
+	template <class F> u64 read_header(F reference) {
+		if (stream) return format == INPUT_BAM ? read_bam_header(*stream, reference) : read_sam_header(*stream, reference);
+		file_source src(f);
+		return format == INPUT_BAM ? read_bam_header(src, reference) : read_sam_header(src, reference);
+	}
+	void drain() { if (stream) stream->drain(); }
 };
 
+static void read_inputs(input_file& chim, input_file& main_file, refdata& ref, const ingest_options& opt, fragment_table& out, coverage_windows& coverage, ingest_stats& stats);
+
 void read_chimeric_alignments(const std::string& bam_path, refdata& ref, const ingest_options& opt, fragment_table& out, coverage_windows& coverage, ingest_stats& stats) {
+	const int T = std::min(255, std::max(1, opt.threads));
+	const u64 chunk_target = getenv("ARB_CHUNK_BYTES") ? (u64) atoll(getenv("ARB_CHUNK_BYTES")) : 128ull << 20; // env: test hook (many small chunks)
+	// A separate chimeric file (-c) is read first, in a call of its own in the reference (arriba.cpp:123-130): its header, then the main file's, name the
+	// contigs (ids in that order; a contig's printed name is the last header's spelling), its records go into the store ahead of the main file's.
+	// A file's framing is checked as it is opened; a stream's as it is read, and after any other error the rest of each stream the file path would have
+	// checked by then is walked, so that a framing error wins as it does for a file.
+	input_file chim, main_file;
+	if (!opt.chimeric_path.empty()) chim.open(opt.chimeric_path, T, chunk_target);
+	try { main_file.open(bam_path, T, chunk_target); } catch (const framing_error&) { throw; } catch (const std::exception&) { chim.drain(); throw; }
+	try { read_inputs(chim, main_file, ref, opt, out, coverage, stats); }
+	catch (const framing_error&) { throw; }
+	catch (const std::exception&) { chim.drain(); main_file.drain(); throw; }
+}
+
+static void read_inputs(input_file& chim, input_file& main_file, refdata& ref, const ingest_options& opt, fragment_table& out, coverage_windows& coverage, ingest_stats& stats) {
 	const int T = std::min(255, std::max(1, opt.threads));
 	const bool trace = getenv("ARB_TRACE") != NULL;
 	double tr_last = now_s();
 	auto lap = [&](const char* what) { if (trace) { const double t = now_s(); fprintf(stderr, "[ingest] %-28s %.3f s\n", what, t - tr_last); tr_last = t; } };
-	const u64 chunk_target = getenv("ARB_CHUNK_BYTES") ? (u64) atoll(getenv("ARB_CHUNK_BYTES")) : 128ull << 20; // env: test hook (many small chunks)
-	// A separate chimeric file (-c) is read first, in a call of its own in the reference (arriba.cpp:123-130): its header, then the main file's, name the
-	// contigs (ids in that order; a contig's printed name is the last header's spelling), its records go into the store ahead of the main file's.
+	const u64 chunk_target = getenv("ARB_CHUNK_BYTES") ? (u64) atoll(getenv("ARB_CHUNK_BYTES")) : 128ull << 20;
 	const bool has_chimeric = !opt.chimeric_path.empty();
-	input_file chim, main_file;
-	if (has_chimeric) { chim.f.map(opt.chimeric_path); chim.format = detect_format(chim.f, T, chunk_target); }
-	main_file.f.map(bam_path); main_file.format = detect_format(main_file.f, T, chunk_target);
 	lap("open + block table");
 	stats.t_inflate = stats.t_parse = stats.t_finalize = 0;
 	stats.chimeric_records = stats.chimeric_malformed = stats.chimeric_total = 0;
@@ -358,14 +518,14 @@ void read_chimeric_alignments(const std::string& bam_path, refdata& ref, const i
 	std::vector<u8> interesting_contig, viral_contig;
 	for (input_file* in : {&chim, &main_file}) {
 		if (in == &chim && !has_chimeric) continue;
-		if (in->f.blocks.empty()) fail("failed to read SAM header");
+		if (!in->has_blocks()) fail("failed to read SAM header");
 		auto add_reference = [&](const std::string& target) { // the next reference of the header (BAM or @SQ)
 			const u16 id = ref.contig_id(remove_chr(target));
 			ref.original_names[id] = target;
 			in->tid_to_contig.push_back(id);
 		};
-		if (in->format != INPUT_BAM) in->header_end = read_sam_header(in->f, [&](const std::string& name) { add_reference(name); in->sq_names += name; in->sq_off.push_back(in->sq_names.size()); });
-		else in->header_end = read_bam_header(in->f, add_reference);
+		if (in->format != INPUT_BAM) in->header_end = in->read_header([&](const std::string& name) { add_reference(name); in->sq_names += name; in->sq_off.push_back(in->sq_names.size()); });
+		else in->header_end = in->read_header(add_reference);
 	}
 	{ // the contig flags of the grown contig table, and the coverage windows
 		const size_t nc = ref.contig_ids.size();
@@ -384,14 +544,20 @@ void read_chimeric_alignments(const std::string& bam_path, refdata& ref, const i
 		std::vector<u64> n_windows(nc);
 		for (u32 c = 0; c < nc; ++c) n_windows[c] = coverage.coverage[c].size();
 		check(arb_records_begin(ctx, main_file.tid_to_contig.data(), (u32) main_file.tid_to_contig.size(), interesting_contig.data(), viral_contig.data(), n_windows.data(), nc,
-		                        opt.max_itd_length, opt.external_duplicate_marking ? 1 : 0, main_file.f.total_out + (has_chimeric ? chim.f.total_out : 0)), "arb_records_begin");
+		                        opt.max_itd_length, opt.external_duplicate_marking ? 1 : 0,
+		                        main_file.stream || chim.stream ? 0 : main_file.f.total_out + (has_chimeric ? chim.f.total_out : 0) /* a stream's size is not known */), "arb_records_begin");
 	}
 	lap("header");
 
 	// chunks of ~128 MiB of decompressed data, each a whole number of BGZF blocks (pieces of a plain SAM file); a record (or line) that straddles a chunk
 	// boundary stays on the device for the next one
-	// A chunk is inflated by the host while the device copies and scans the previous one.
-	struct chunk_t { column<u8> buf /* page-locked: copied to the device asynchronously */; u64 pos /* in the inflated stream */; u64 first; bool last; chunk_t(): pos(0), first(0), last(false) {} };
+	// A chunk is inflated by the host while the device copies and scans the previous one. A stream's chunk is read while the device scans the previous one:
+	// the producer keeps writing, and waits only when both buffers are full.
+	struct chunk_t {
+		column<u8> buf /* page-locked: copied to the device asynchronously */; u64 pos /* in the inflated stream */; u64 first; bool last;
+		u64 bytes /* stream: the inflated bytes of the chunk */, raw_bytes /* BGZF stream: the bytes of buf that go up */; std::vector<arb_bgzf_block> blocks /* BGZF stream */;
+		chunk_t(): pos(0), first(0), last(false), bytes(0), raw_bytes(0) {}
+	};
 	chunk_t chunks[2];
 	double t_inflate = 0; // written by the inflating thread only
 	const u64 NO_ERROR = ~(u64) 0;
@@ -414,21 +580,94 @@ void read_chimeric_alignments(const std::string& bam_path, refdata& ref, const i
 			c.last = b0 >= bam.blocks.size(); c.first = 0;
 			t_inflate += now_s() - ti;
 		};
-		while (b0 < bam.blocks.size() && bam.blocks[b0].out_off + bam.blocks[b0].out_len <= in.header_end) ++b0; // the first chunk starts at the block of the first record
-		prepare(chunks[0]);
+		// A stream's chunk: the bytes left behind the previous chunk, then read(). BGZF: the same whole blocks the file path's chunk would hold (the block
+		// that does not fit stays for the next chunk); stored blocks stay where they were read, the others are inflated behind the read bytes, and the
+		// block table says where each payload is. Plain SAM: the bytes of the file path's chunk (a whole number of its pieces).
+		auto prepare_stream = [&](chunk_t& c) {
+			const double ti = now_s();
+			stream_input& s = *in.stream;
+			column<u8>& buf = c.buf;
+			const u64 piece = input_file::piece(chunk_target), text_bytes = std::max<u64>(1, chunk_target / piece) * piece;
+			const size_t base = (size_t) std::min<u64>(s.bgzf ? chunk_target : text_bytes, 1ull << 30) + (1u << 20);
+			if (buf.capacity() < base) buf.reserve(base);
+			buf.resize(std::max(buf.capacity(), std::max(base, s.n_left)));
+			size_t have = s.n_left;
+			memcpy(buf.data(), s.left, have);
+			auto read_more = [&](size_t want) { // false at the end of the stream
+				if (buf.size() - have < want) buf.resize(have + want);
+				if (want == 0) return true;
+				const size_t got = s.read_some(buf.data() + have, want);
+				have += got; return got > 0;
+			};
+			c.pos = s.out_pos; c.first = 0; c.last = false; c.blocks.clear();
+			if (!s.bgzf) {
+				while (have < text_bytes + 1 && read_more(std::min<size_t>(buf.size() - have, (size_t) text_bytes + (64u << 10) - have))) {} // one byte beyond tells whether this is the last chunk
+				c.bytes = std::min<u64>(have, text_bytes); c.last = have <= text_bytes;
+				s.left = buf.data() + c.bytes; s.n_left = have - c.bytes; s.out_pos += c.bytes;
+				t_inflate += now_s() - ti;
+				return;
+			}
+			size_t at = 0; u64 bytes = 0;
+			std::vector<u32> in_len;
+			for (;;) {
+				u32 bsize = 0, xlen = 0;
+				const int r = stream_block_at(buf.data() + at, have - at, s.eof, bsize, xlen);
+				if (r < 0) { c.last = true; break; }
+				if (r == 0) { // the rest of the chunk is estimated from its ratio of read to inflated bytes so far
+					const double ratio = bytes ? std::min(1.0, (double) at / (double) bytes) : 1.0;
+					const size_t want = (size_t) std::min<double>((double) (chunk_target > bytes ? chunk_target - bytes : 0) * ratio, (double) (1u << 30)) + (64u << 10) + 64;
+					read_more(want);
+					continue;
+				}
+				const u32 out_len = rd32(buf.data() + at + bsize - 4);
+				if (bytes != 0 && bytes + out_len > chunk_target) break;
+				const arb_bgzf_block b = {at + 12 + xlen, out_len, bytes};
+				c.blocks.push_back(b); in_len.push_back(bsize - 20 - xlen);
+				bytes += out_len; at += bsize;
+			}
+			// the payloads: stored ones in place, the others inflated behind the bytes read
+			std::vector<size_t> packed; std::vector<u64> deflate_at; u64 inflated = 0;
+			for (size_t k = 0; k < c.blocks.size(); ++k) {
+				arb_bgzf_block& b = c.blocks[k];
+				if (b.bytes == 0) continue;
+				if (stored_block(buf.data() + b.src, in_len[k], (u32) b.bytes)) { b.src += 5; continue; }
+				packed.push_back(k); deflate_at.push_back(b.src); b.src = have + inflated; inflated += b.bytes;
+			}
+			if (buf.size() < have + inflated) buf.resize(have + inflated);
+			s.left = buf.data() + at; s.n_left = have - at; s.out_pos += bytes;
+			c.bytes = bytes; c.raw_bytes = packed.empty() ? at : have + inflated;
+			parallel_for(T, packed.size(), [&](int, size_t lo, size_t hi) {
+				for (size_t j = lo; j < hi; ++j) { const arb_bgzf_block& b = c.blocks[packed[j]]; inflate_payload(buf.data() + deflate_at[j], in_len[packed[j]], (u32) b.bytes, buf.data() + b.src); }
+			});
+			t_inflate += now_s() - ti;
+		};
+		if (in.stream) { in.stream->header_done(in.header_end, input_file::piece(chunk_target)); prepare_stream(chunks[0]); }
+		else {
+			while (b0 < bam.blocks.size() && bam.blocks[b0].out_off + bam.blocks[b0].out_len <= in.header_end) ++b0; // the first chunk starts at the block of the first record
+			prepare(chunks[0]);
+		}
 		chunks[0].first = in.header_end - chunks[0].pos;
 		if (in.format != INPUT_BAM) check(arb_records_text_names(ctx, in.sq_names.data(), in.sq_off.data(), (u32) in.tid_to_contig.size()), "arb_records_text_names");
 		u64 total_records = 0;
 		for (int cur = 0;; cur ^= 1) {
 			chunk_t& c = chunks[cur];
-			std::string prepare_error; std::thread next;
-			if (!c.last) next = std::thread([&]() { try { prepare(chunks[cur ^ 1]); } catch (const std::exception& x) { prepare_error = x.what(); if (prepare_error.empty()) prepare_error = "failed to load alignments"; } });
+			std::string prepare_error; bool prepare_framing = false; std::thread next;
+			if (!c.last) next = std::thread([&]() {
+				try { if (in.stream) prepare_stream(chunks[cur ^ 1]); else prepare(chunks[cur ^ 1]); }
+				catch (const framing_error& x) { prepare_error = x.what(); prepare_framing = true; }
+				catch (const std::exception& x) { prepare_error = x.what(); if (prepare_error.empty()) prepare_error = "failed to load alignments"; }
+			});
 			const double tp = now_s();
 			uint64_t n_records = 0, carry = 0, error = NO_ERROR; uint32_t malformed = 0;
-			const int rc = in.format == INPUT_BAM ? arb_records_chunk(ctx, c.buf.data(), c.buf.size(), c.first, c.pos, &n_records, &carry, &malformed, &error)
-			                                      : arb_records_text_chunk(ctx, c.buf.data(), c.buf.size(), c.first, c.pos, c.last ? 1 : 0, &n_records, &carry, &error);
+			const u8* data = c.buf.data(); u64 bytes = c.buf.size();
+			int rc = 0;
+			if (in.stream) bytes = c.bytes;
+			if (in.stream && in.stream->bgzf) { rc = arb_records_bgzf_stage(ctx, c.buf.data(), c.raw_bytes, c.blocks.data(), (u32) c.blocks.size()); data = NULL; }
+			if (rc == 0) rc = in.format == INPUT_BAM ? arb_records_chunk(ctx, data, bytes, c.first, c.pos, &n_records, &carry, &malformed, &error)
+			                                         : arb_records_text_chunk(ctx, data, bytes, c.first, c.pos, c.last ? 1 : 0, &n_records, &carry, &error);
 			stats.t_parse += now_s() - tp;
 			if (next.joinable()) next.join();
+			if (prepare_framing) throw framing_error(prepare_error); // a file's framing is checked before any record
 			check(rc, in.format == INPUT_BAM ? "arb_records_chunk" : "arb_records_text_chunk");
 			if (malformed) fail("failed to load alignments");
 			total_records += n_records;
@@ -438,14 +677,20 @@ void read_chimeric_alignments(const std::string& bam_path, refdata& ref, const i
 		}
 		return total_records;
 	};
-	if (has_chimeric) {
-		u64 first = 0;
-		check(arb_records_source(ctx, 1, chim.tid_to_contig.data(), (u32) chim.tid_to_contig.size(), &first), "arb_records_source");
-		stats.chimeric_records = read_records(chim);
-		if (record_error == NO_ERROR) check(arb_records_source(ctx, 0, main_file.tid_to_contig.data(), (u32) main_file.tid_to_contig.size(), &main_first), "arb_records_source");
-		else main_first = NO_ERROR; // the main file is not read
-	}
-	stats.records = record_error == NO_ERROR ? read_records(main_file) : 0;
+	try {
+		if (has_chimeric) {
+			u64 first = 0;
+			check(arb_records_source(ctx, 1, chim.tid_to_contig.data(), (u32) chim.tid_to_contig.size(), &first), "arb_records_source");
+			stats.chimeric_records = read_records(chim);
+			if (record_error == NO_ERROR) check(arb_records_source(ctx, 0, main_file.tid_to_contig.data(), (u32) main_file.tid_to_contig.size(), &main_first), "arb_records_source");
+			else main_first = NO_ERROR; // the main file is not read
+		}
+		stats.records = record_error == NO_ERROR ? read_records(main_file) : 0;
+	} catch (const framing_error&) { throw; } catch (const std::exception&) { chim.drain(); main_file.drain(); throw; }
+	// The records stop here (a record error, or the end of the input). A stream's framing error further on outranks whatever follows -- the replay's
+	// errors, the -c file's warning and progress line -- as it does for a file, whose framing is checked when it is opened; and the chunk buffers the
+	// streams' unread bytes lie in are still alive.
+	chim.drain(); main_file.drain();
 	if (trace) fprintf(stderr, "[ingest]   of which inflate %.3f s (overlaps with) chunk copies + record extraction %.3f s\n", t_inflate, stats.t_parse);
 	stats.t_inflate = t_inflate;
 	{ chunk_t a, b; std::swap(chunks[0], a); std::swap(chunks[1], b); }
@@ -476,6 +721,11 @@ void read_chimeric_alignments(const std::string& bam_path, refdata& ref, const i
 		const bool in_chimeric_file = has_chimeric && (record_error >> 3) < main_first;
 		if (has_chimeric && !in_chimeric_file) chimeric_file_done();
 		fail(record_error_text(record_error, ctx, in_chimeric_file ? chim.tid_to_contig : main_file.tid_to_contig, ref));
+	}
+	if (trace) {
+		arb_timings tm;
+		if (arb_get_timings(ctx, &tm) == 0)
+			fprintf(stderr, "[ingest]   record store: allocated %u times, %.1f MB at most; %.1f MB copied to the device, %.1f ms assembling stream chunks\n", tm.rec_store_grows, tm.rec_store_bytes / 1e6, tm.rec_h2d_bytes / 1e6, tm.rec_unwrap_ms);
 	}
 	lap("replay (device)");
 	stats.mapped_reads = counters[REC_CTR_MAPPED]; stats.malformed = counters[REC_CTR_MALFORMED]; stats.missing_hi_tag = counters[REC_CTR_MISSING_HI];

@@ -1,6 +1,8 @@
 // records.cu -- the reference's record loop on the device (functors: records_hd.h).
 //   records_begin  : the BAM header's contig map, the contig flags, the coverage windows' layout,
 //   records_source : a separate chimeric file (-c) ahead of the main file: which file the following chunks belong to, and its header's contig map,
+//   records_bgzf_stage : stream input: the raw BGZF blocks of a chunk go up as they were read, and the inflated chunk is assembled on the device
+//                    (stage_hd.h) where records_upload would have put it,
 //   records_chunk  : per chunk of inflated payload: copy it up behind the unfinished record of the previous chunk, find the records (bamscan.cu), classify
 //                    them and append the kept ones to the record store, which lives across chunks (mates and supplementaries of one key may sit anywhere
 //                    in the file),
@@ -13,6 +15,7 @@
 #include "engine.h"
 #include "records_hd.h"
 #include "fragtable_hd.h"
+#include "stage_hd.h"
 
 namespace arb {
 
@@ -62,6 +65,8 @@ void engine::records_begin(const u16* tid_to_contig, u32 n_tid, const u8* intere
 	rec_hash_mask = bits && atoi(bits) > 0 && atoi(bits) < 64 ? ((u64) 1 << atoi(bits)) - 1 : ~(u64) 0;
 	timings.bam_scan_ms = 0; timings.h2d_ms = 0; timings.h2d_bytes = 0;
 	timings.rec_chunk_copy_ms = timings.rec_chunk_kernels_ms = timings.rec_sort_ms = timings.rec_count_ms = timings.rec_scan_ms = timings.rec_write_ms = timings.rec_download_ms = timings.rec_text_parse_ms = 0;
+	timings.rec_unwrap_ms = 0; timings.rec_store_grows = 0; timings.rec_store_bytes = 0; timings.rec_h2d_bytes = 0;
+	rec_stage_pending = false; rec_staged = 0;
 	rec_open = true;
 }
 
@@ -76,11 +81,18 @@ void engine::records_source(bool chimeric_file, const u16* tid_to_contig, u32 n_
 	rec_has_chimeric = rec_has_chimeric || chimeric_file; rec_src_chimeric = chimeric_file;
 	rec_pos_base = rec_pos_end; *first_position = rec_pos_base;
 	rec_n_tid = n_tid; rec_tid.upload(ex, tid_to_contig, n_tid); rec_tid.ensure(1);
-	rec_text_staged = 0; rec_carry_at = 0;
+	rec_text_staged = 0; rec_carry_at = 0; rec_stage_pending = false;
 }
 
-// the chunk goes to the device behind the unfinished record (or line) at the end of the previous one; returns the bytes of bam_buf now in use
+// the chunk goes to the device behind the unfinished record (or line) at the end of the previous one; returns the bytes of bam_buf now in use. chunk ==
+// NULL: the chunk records_bgzf_stage put there (without one, NULL with 0 bytes stays an empty chunk).
 u64 engine::records_upload(const u8* chunk, u64 bytes) {
+	if (!chunk && (rec_stage_pending || bytes != 0)) {
+		if (!rec_stage_pending || bytes != rec_staged) throw arb_error("a NULL chunk takes the chunk of arb_records_bgzf_stage, and as many bytes as it staged");
+		rec_stage_pending = false;
+		return rec_carry + bytes;
+	}
+	if (rec_stage_pending) throw arb_error("the chunk of arb_records_bgzf_stage has not been read (pass chunk = NULL)");
 	const u64 total = rec_carry + bytes;
 	if (total >= 0xFFFFFFF0ull) throw arb_error("failed to load alignments (chunk too large)");
 	bam_buf_next.ensure(total + 64);
@@ -92,8 +104,36 @@ u64 engine::records_upload(const u8* chunk, u64 bytes) {
 #endif
 	}
 	bam_buf_next.upload_at(ex, chunk, bytes, rec_carry);
+	timings.rec_h2d_bytes += bytes;
 	bam_buf.swap(bam_buf_next);
 	return total;
+}
+
+void engine::records_bgzf_stage(const u8* raw, u64 raw_bytes, const arb_bgzf_block* blocks, u32 n_blocks) {
+	if (!rec_open) throw arb_error("arb_records_bgzf_stage without arb_records_begin");
+	if (rec_stage_pending) throw arb_error("arb_records_bgzf_stage: the chunk staged before has not been read");
+	if (raw_bytes && !raw) throw arb_error("arb_records_bgzf_stage: no raw bytes");
+	u64 out = 0;
+	for (u32 k = 0; k < n_blocks; ++k) {
+		if (blocks[k].dst != out || blocks[k].src > raw_bytes || blocks[k].bytes > raw_bytes - blocks[k].src) throw arb_error("arb_records_bgzf_stage: block " + std::to_string(k) + " is out of place or outside the raw bytes");
+		out += blocks[k].bytes;
+	}
+	const u64 total = rec_carry + out;
+	if (total >= 0xFFFFFFF0ull) throw arb_error("failed to load alignments (chunk too large)");
+	stage_timer t_all(ex), t_copy(ex);
+	rec_raw.ensure(raw_bytes); rec_raw.upload_at(ex, raw, raw_bytes, 0);
+	rec_stage_blocks.upload(ex, blocks, n_blocks); rec_stage_blocks.ensure(1);
+	timings.rec_h2d_bytes += raw_bytes + (u64) n_blocks * sizeof(arb_bgzf_block);
+	timings.rec_chunk_copy_ms += t_copy.stop();
+	stage_timer t_unwrap(ex);
+	bam_buf_next.ensure(total + 64);
+	const stage_gather_fn g = {bam_buf.ptr() + rec_carry_at, rec_carry, rec_raw.ptr(), rec_stage_blocks.ptr(), n_blocks, total, bam_buf_next.ptr()};
+	for_each(ex, (u32) ((total + 15) / 16), g);
+	bam_buf.swap(bam_buf_next);
+	rec_carry_at = 0; rec_staged = out; rec_stage_pending = true;
+	const float ms = t_unwrap.stop();
+	timings.rec_unwrap_ms += ms; timings.rec_chunk_kernels_ms += ms;
+	timings.bam_scan_ms += t_all.stop();
 }
 
 void engine::records_chunk(const u8* chunk, u64 bytes, u64 first, u64 chunk_pos, u64* n_records, u64* carry, u32* malformed, u64* error) {
@@ -142,6 +182,8 @@ void engine::records_store(const dbuf<u8>& B, u64 buf_pos, u64 total, const u32*
 		try {
 			grow_keep(ex, rec_arena, rec_arena_used, want_bytes); grow_keep(ex, rec_at, rec_n, want_items); grow_keep(ex, rec_pos, rec_n, want_items);
 			grow_keep(ex, rec_hash_lo, rec_n, want_items); grow_keep(ex, rec_hash_hi, rec_n, want_items); grow_keep(ex, rec_hit, rec_n, want_items); grow_keep(ex, rec_sa, rec_n, want_items);
+			++timings.rec_store_grows;
+			timings.rec_store_bytes = std::max<u64>(timings.rec_store_bytes, (u64) rec_arena.size() + (u64) rec_at.size() * (8 + 8 + 4 + 4 + 8 + 1));
 		} catch (const arb_error& e) {
 			char m[256];
 			snprintf(m, sizeof(m), "the BAM record store does not fit in device memory: %llu records in %.2f GB (%s)", (unsigned long long) want_items,

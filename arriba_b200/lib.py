@@ -71,7 +71,8 @@ class Timings(C.Structure):
                 ("rec_chunk_copy_ms", C.c_float), ("rec_chunk_kernels_ms", C.c_float), ("rec_sort_ms", C.c_float), ("rec_count_ms", C.c_float),
                 ("rec_scan_ms", C.c_float), ("rec_write_ms", C.c_float), ("rec_download_ms", C.c_float),
                 ("rec_text_parse_ms", C.c_float), ("fill_gaps_ms", C.c_float),
-                ("fill_gaps_jobs", C.c_uint64), ("fill_gaps_chars", C.c_uint64)]
+                ("fill_gaps_jobs", C.c_uint64), ("fill_gaps_chars", C.c_uint64),
+                ("rec_unwrap_ms", C.c_float), ("rec_store_grows", C.c_uint32), ("rec_store_bytes", C.c_uint64), ("rec_h2d_bytes", C.c_uint64)]
 
 
 _CTYPE = {np.dtype(np.uint8): C.c_uint8, np.dtype(np.uint16): C.c_uint16, np.dtype(np.uint32): C.c_uint32, np.dtype(np.int32): C.c_int32,
@@ -578,7 +579,9 @@ class Pipeline:
     """One run of the hot path on files: the call a user of the library makes (the `arriba` CLI is a thin wrapper over it).
 
     `bam` is the alignment file: BAM, or SAM text (plain or BGZF-compressed), told apart by the content (DESIGN.md section 5). `chimeric` is STAR's
-    separate chimeric alignment file (Chimeric.out.sam, from --chimOutType SeparateSAMold; any of the same formats), read before `bam` (the -c option)."""
+    separate chimeric alignment file (Chimeric.out.sam, from --chimOutType SeparateSAMold; any of the same formats), read before `bam` (the -c option).
+    Either may be a regular file or a path that reads as a stream: a pipe or FIFO ("/dev/stdin", "/dev/fd/N", os.mkfifo) or a character device. A stream
+    is read once, in order, while the records are processed; it gives the same results as the same bytes in a file."""
 
     def __init__(self, bam, gtf, fasta, threads=1, device=0, lib_path=None, strandedness=3, params=None, output=None, discarded=None,
                  genomic_breakpoints=None, max_genomic_breakpoint_distance=100000, blacklist=None, known_fusions=None, tags=None, protein_domains=None,

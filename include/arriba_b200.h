@@ -114,7 +114,8 @@ int arb_push_chunk_end(arb_ctx* ctx, const arb_soa_chunk* chunk);
  * supplementaries of one read may sit anywhere in the file), then groups them by "<qname>,<HI>" and replays the loop in file order into the fragment pools.
  *   arb_records_begin  : tid_to_contig = contig id of every BAM reference (n_tid); interesting / viral contig flags and the number of 20-bp coverage windows
  *                        per contig (n_contigs = the contigs of arb_set_contigs, which must have been called with the grown table; the gene index of
- *                        arb_set_annotation is the one the read-through test queries); expected_bytes = the inflated size of the file (sizes the store),
+ *                        arb_set_annotation is the one the read-through test queries); expected_bytes = the inflated size of the file (sizes the store
+ *                        from the first chunk; 0 = unknown, e.g. input from a pipe: the store then grows by a quarter whenever it is full),
  *   arb_records_chunk  : one chunk of inflated payload (page-locked host memory makes the copy asynchronous). chunk_pos = its position in the inflated
  *                        stream; first = offset of the first record (behind the header) in the first chunk, else 0. The unfinished record at the end of a
  *                        chunk is kept on the device for the next one: carry = its bytes (not 0 after the last chunk: truncated file). malformed != 0:
@@ -160,6 +161,17 @@ int arb_records_finish(arb_ctx* ctx, uint16_t* const* coverage, uint8_t* const* 
  *                            The bytes after the last LF are kept for the next chunk (carry); with last != 0 they are the last line. error: as for
  *                            arb_records_chunk, with positions in the stream of staged records, which keeps file order; an unreadable line is an error of
  *                            kind 1. arb_records_error_record hands out the staged body. arb_records_finish follows as for BAM input. */
+/* A BGZF stream read from a pipe (DESIGN.md section 5, "Stream input") is not inflated on the host: the chunk goes up as it was read, and the device
+ * assembles the inflated payload.
+ *   arb_records_bgzf_stage : raw = whole BGZF blocks as read, followed by the host's inflated copies of the blocks that are really compressed (page-locked
+ *                            memory makes the copy asynchronous; raw may be NULL when raw_bytes is 0). blocks[k] = {src, bytes, dst}: the payload of block
+ *                            k is `bytes` bytes at raw + src and goes to offset dst of the inflated chunk; dst of block 0 is 0 and every block starts where
+ *                            the one before it ends (empty blocks included). The device places the assembled chunk behind the carried unfinished record.
+ *                            Then arb_records_chunk or arb_records_text_chunk with chunk = NULL and bytes = the chunk's inflated size takes the staged chunk
+ *                            (without a staged chunk, NULL with bytes = 0 is an empty chunk, as before).
+ */
+typedef struct { uint64_t src, bytes, dst; } arb_bgzf_block;
+int arb_records_bgzf_stage(arb_ctx* ctx, const uint8_t* raw, uint64_t raw_bytes, const arb_bgzf_block* blocks, uint32_t n_blocks);
 int arb_records_source(arb_ctx* ctx, int chimeric_file, const uint16_t* tid_to_contig, uint32_t n_tid, uint64_t* first_position);
 int arb_records_text_names(arb_ctx* ctx, const char* names, const uint64_t* name_off, uint32_t n_names);
 int arb_records_text_chunk(arb_ctx* ctx, const uint8_t* chunk, uint64_t bytes, uint64_t first, uint64_t chunk_pos, int last, uint64_t* n_records, uint64_t* carry, uint64_t* error);
@@ -473,6 +485,10 @@ typedef struct arb_timings {
 	float rec_text_parse_ms;    /* SAM input, part of rec_chunk_kernels_ms: line ends, the parse and the staged BAM records, summed over the chunks */
 	float fill_gaps_ms;         /* -I: arb_set_fill_transcripts plus every arb_fill_gaps since (copies of the jobs, plan, scan and the filled sequences) */
 	uint64_t fill_gaps_jobs, fill_gaps_chars; /* -I: the jobs of every arb_fill_gaps and the characters they wrote */
+	float rec_unwrap_ms;        /* stream input, part of rec_chunk_kernels_ms: arb_records_bgzf_stage's assembly of the inflated chunks, summed over the chunks */
+	uint32_t rec_store_grows;   /* the record loop of the last sample: how often the record store was (re)allocated */
+	uint64_t rec_store_bytes;   /* its largest size in bytes (records and per-record columns) */
+	uint64_t rec_h2d_bytes;     /* bytes the record loop copied host->device: the chunks (stream input: the raw chunks and their block tables) */
 } arb_timings;
 int arb_get_timings(arb_ctx* ctx, arb_timings* out);
 /* Device scratch memory is pooled per device and survives arb_ctx_destroy so that the next sample reuses it; this returns it to the driver
@@ -487,7 +503,7 @@ void arb_release_host_memory(void);
  * stages above. Host work is C++ on `threads` host threads; all device work goes through the entry points above. */
 typedef struct arb_pipeline arb_pipeline;
 typedef struct arb_run_options {
-	const char* bam_file;            /* -x */
+	const char* bam_file;            /* -x: a regular file, or a pipe, FIFO or character device read sequentially (e.g. "/dev/stdin") */
 	const char* gtf_file;            /* -g */
 	const char* assembly_file;       /* -a */
 	const char* output_file;         /* -o (may be NULL until the writer stage is requested) */
@@ -517,7 +533,7 @@ typedef struct arb_run_options {
 	const char* known_fusions_file;  /* -k: known fusions (optionally .gz), NULL = none; read only while the known_fusions filter is on */
 	const char* tags_file;           /* -t: tags (optionally .gz), NULL = none */
 	const char* protein_domains_file; /* -p: protein domains (GFF3, optionally .gz), NULL = none */
-	const char* chimeric_file;       /* -c: STAR's Chimeric.out.sam (SAM, BGZF SAM or BAM; --chimOutType SeparateSAMold), NULL = none */
+	const char* chimeric_file;       /* -c: STAR's Chimeric.out.sam (SAM, BGZF SAM or BAM; --chimOutType SeparateSAMold; a file or a pipe, as -x), NULL = none */
 	int32_t fill_sequence_gaps;      /* -I */
 } arb_run_options;
 void arb_default_run_options(arb_run_options* o);
